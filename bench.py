@@ -5,9 +5,9 @@
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" is one pass of the hot path -- mu.atac.pp.tfidf + mu.atac.tl.lsi -- over the whole synthetic matrix.
-Default workload = BASELINE.json configs[1]: 1M cells x 200k peaks, 3 % nnz per GPU (weak scaling: every rank owns
-1M cells; peak-space objects are replicated, one allreduce of column sums, one of A^T Y per Lanczos step, one of
-the b x b Gram per QR).  ``--scaling strong`` splits --cells over the ranks instead.
+Default workload = BASELINE.json configs[1]: 500k cells x 200k peaks, 3 % nnz per GPU (3e9 non-zeros; ~62 GB of HBM at
+the peak of a step, so that it fits one 80 GB H100).  Weak scaling: every rank owns 500k cells; peak-space objects are
+replicated, one allreduce of column sums, one of A^T Y per Lanczos step, one of the b x b Gram per QR.  ``--scaling strong`` splits --cells over the ranks instead.
 
 Prints ONE JSON line (rank 0):
   value        cells/s with the counts already resident in HBM (CUDA events, max over ranks)
@@ -17,7 +17,9 @@ Prints ONE JSON line (rank 0):
   cpu_baseline the scipy oracle on a bounded row-sample + the GPU on that SAME sample (same_matrix_speedup)
   mofa         BASELINE configs[2]: mu.tl.mofa, RNA + ATAC, k=30, 15 iterations, cells sharded like the main leg
   strong       (N > 1) the main step with --cells TOTAL split over the ranks
-  cfg3         (N = 8, or --cfg3 1) BASELINE configs[3]: LSI k=100 on 4M x 500k over 8 GPUs
+  cfg3         (N = 8, or --cfg3 1) BASELINE configs[3]: LSI k=100 on 2M x 500k over 8 GPUs
+``--dump-outputs DIR`` writes what the main leg's last timed step returned (TF-IDF values, LSI embedding, loadings and
+stdev; fixed seeded samples of the large arrays) as DIR/<name>.npy, so that two builds can be compared output for output.
 ``--impl reference`` times the CPU oracle (scipy restatement of the reference, oracle/) on the host cores; it never
 loads the CUDA library.
 """
@@ -38,7 +40,7 @@ if ROOT not in sys.path:
 
 import numpy as np  # noqa: E402
 
-METRIC = "cells/sec for TF-IDF+LSI(k=50) on 1Mx200k sparse ATAC"
+METRIC = "cells/sec for TF-IDF+LSI(k=50) on 500kx200k sparse ATAC"
 
 
 def parse():
@@ -48,7 +50,7 @@ def parse():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
-    ap.add_argument("--cells", type=int, default=1_000_000, help="cells per GPU (weak) or in total (strong)")
+    ap.add_argument("--cells", type=int, default=500_000, help="cells per GPU (weak) or in total (strong)")
     ap.add_argument("--peaks", type=int, default=200_000)
     ap.add_argument("--density", type=float, default=0.03)
     ap.add_argument("--k", type=int, default=50)
@@ -72,12 +74,14 @@ def parse():
     ap.add_argument("--mofa-iters", type=int, default=15)
     ap.add_argument("--mofa-k", type=int, default=30)
     ap.add_argument("--breakdown", action="store_true", help="one extra, synchronising step with phase timers")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the main leg's last-step outputs as DIR/<name>.npy (float32/float64, < 64 MB in all)")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (sampled every 200 ms)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -115,7 +119,7 @@ class ClockSampler:
                 "reasons": reasons, "samples": len(sm)}
 
 
-def onchip_roofline(nnz, P, ms_per_pass, sm_mhz, n_sms=148, operand_bytes=4.0):
+def onchip_roofline(nnz, P, ms_per_pass, sm_mhz, n_sms=132, operand_bytes=4.0):
     """Second roofline of the SpMM kernel: every non-zero moves P operand elements plus its 8-byte {index, value}
     entry through the SM's L1/LSU data path (128 B/clk/SM, shared with shared-memory traffic).  Reported next to
     the HBM figure because this, not DRAM, is what the kernel saturates (DESIGN.md section 4)."""
@@ -128,11 +132,14 @@ def onchip_roofline(nnz, P, ms_per_pass, sm_mhz, n_sms=148, operand_bytes=4.0):
             "frac": ach / peak, "bytes_per_nnz": operand_bytes * P + 8.0, "sm_mhz": sm_mhz, "sms": n_sms}
 
 
+HBM_DATASHEET_GBS = 3350.0      # H100 SXM data sheet (HBM3); not a measured figure
+
+
 def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": HBM_DATASHEET_GBS}, "datasheet"
 
 
 def host_threads():
@@ -236,14 +243,52 @@ def lsi_step_fn(ctx, A, k, tol):
     var0 = pd.DataFrame(index=pd.RangeIndex(A.shape[1]).astype(str))
 
     def step():
+        step.last = None                              # the previous step's AnnData goes before this one allocates
         ad = mu.SimpleAnnData(A, obs=obs0, var=var0)  # counts stay untouched: tfidf writes a new matrix
         mu.atac.pp.tfidf(ad)
         info = mu.atac.tl.lsi(ad, n_comps=k, tol=tol, return_info=True)
         # leading singular values (stdev * sqrt(n-1), tools.py:65): the same global matrix must give the same
         # values on any number of GPUs (strong leg at N ranks vs main leg at 1 rank)
         info.sigma_head = [float(x) * float(np.sqrt(max(A.n_total - 1, 1))) for x in ad.uns["lsi"]["stdev"][:4]]
+        step.last = ad
         return info
+    step.last = None
     return step
+
+
+DUMP_ROWS = 16384          # sampled rows of X_lsi / LSI
+DUMP_NNZ = 1 << 20         # sampled entries of the TF-IDF values
+
+
+def dump_outputs(ad, out_dir, seed=1234):
+    """What mu.atac.pp.tfidf + mu.atac.tl.lsi returned to the caller, as float32/float64 .npy files (about 20 MB at the
+    default sizes).  Large arrays are sampled at positions drawn from a fixed seed that depends only on their shapes,
+    so two builds run with the same arguments write comparable files.  Row / entry positions are stored as float64
+    (exact below 2^53).  Singular vectors are defined up to sign; compare them after aligning signs per column."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(seed)
+    X = ad.X
+    nnz = int(X.nnz)
+    pos = np.unique(rng.integers(0, nnz, size=min(DUMP_NNZ, nnz), dtype=np.int64)) if nnz else np.zeros(0, np.int64)
+    pos_d = torch.from_numpy(pos).to(X.data.device)
+    out = {"tfidf_sample_pos": pos.astype(np.float64),
+           "tfidf_sample_values": X.data[pos_d].cpu().numpy(),
+           "tfidf_sample_indices": X.indices[pos_d].long().cpu().numpy().astype(np.float64),
+           "lsi_stdev": np.asarray(ad.uns["lsi"]["stdev"])}
+    for name, M in (("X_lsi", ad.obsm["X_lsi"]), ("LSI", ad.varm["LSI"])):
+        M = np.asarray(M)
+        rows = np.sort(rng.choice(M.shape[0], size=min(DUMP_ROWS, M.shape[0]), replace=False))
+        out[f"{name}_sample_rows"] = rows.astype(np.float64)
+        out[f"{name}_sample"] = M[rows]
+    total = 0
+    for name, a in out.items():
+        if a.dtype not in (np.float32, np.float64):
+            a = a.astype(np.float64)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        total += a.nbytes
+    assert total <= 64 << 20, total
+    return sorted(out)
 
 
 def spmm_roofline(ctx, kern, info, steps, nnz, n_local, D, k, clocks):
@@ -260,7 +305,7 @@ def spmm_roofline(ctx, kern, info, steps, nnz, n_local, D, k, clocks):
     n_lowp = getattr(info, "lowp_passes", 0) * steps
     total = float(np.sum(f32_ms) + np.sum(h16_ms)) if (f32_ms or h16_ms) else float("nan")
     pk, pk_kind = peaks()
-    hbm = float(pk.get("hbm_gbs", 6650.0))
+    hbm = float(pk.get("hbm_gbs", HBM_DATASHEET_GBS))
     ach = n_pass * pass_bytes / (total * 1e-3) / 1e9 if total == total else None
     r = {"bound": "hbm",
          "kernel": f"spmm_csr_rowwarp_kernel<{P},*> + spmm_csr_rowwarp_h_kernel<{P},*> (A*V on CSR arrays, A^T*U on pair-layout panels)",
@@ -272,14 +317,6 @@ def spmm_roofline(ctx, kern, info, steps, nnz, n_local, D, k, clocks):
          "note": "algorithmic bytes = 8 B/nnz + 4*P*(n+D) per pass; every nnz also gathers P operand elements "
                  "through L2->L1 (4 B each in the fp32 kernel, 2 B in the half-operand kernel), which is the practical "
                  "limiter (DESIGN.md section 4)"}
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        key = f"spmm_rowwarp{P}_n{n_local}_d{D}"
-        if key in tr:
-            r["traffic"] = tr[key]["dram_bytes_per_pass"]
-            r["traffic_source"] = tr[key]["source"]
-    except Exception:
-        pass
     if ctx.rank == 0 and clocks and total == total:
         import torch
         sms = torch.cuda.get_device_properties(ctx.local).multi_processor_count
@@ -355,10 +392,12 @@ def main():
     # ---- main leg: device-resident counts -> tfidf -> lsi ------------------------------------------------------
     step = lsi_step_fn(ctx, A, k, args.tol)
     ms_total, kern, launches, info, clocks = timed_steps(ctx, step, args.steps, args.warmup, sample_clocks=True)
+    dumped = dump_outputs(step.last, args.dump_outputs) if (args.dump_outputs and rank == 0) else None
+    step.last = None
     value = n_total * args.steps / (ms_total / 1e3)
     roofline = spmm_roofline(ctx, kern, info, args.steps, nnz, n_local, D, k, clocks)
     pk, _ = peaks()
-    hbm = float(pk.get("hbm_gbs", 6650.0))
+    hbm = float(pk.get("hbm_gbs", HBM_DATASHEET_GBS))
     tf_red = kern.get("mub_tfidf_reduce_f32", []) + kern.get("mub_tfidf_reduce_tiled_f32", [])
     tf_app = kern.get("mub_tfidf_apply_f32", [])
     if tf_red and tf_app:
@@ -520,6 +559,7 @@ def main():
                                "residual_history": [float("%.3g" % h) for h in info.history]}},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "roofline": roofline, "cpu_baseline": cpu,
             "phase_ms_per_step": phase_ms, "breakdown_ms": breakdown, "strong": strong, "mofa": mofa, "cfg3": cfg3,
+            "dumped_outputs": dumped,
         }
         print(json.dumps(out))
     if world > 1:
@@ -562,7 +602,7 @@ def mofa_leg(ctx, args, box, tb, n_local, n_total, free):
     # SURVEY 8d: per iteration and view two sparse passes of 8 B/nnz + the dense operands once
     spmm_bytes = sum(2 * (8.0 * z + 4.0 * P * (nm + v.shape[1])) for z, v in zip(nnzs, views)) * iters
     pk, pk_kind = peaks()
-    hbm = float(pk.get("hbm_gbs", 6650.0))
+    hbm = float(pk.get("hbm_gbs", HBM_DATASHEET_GBS))
     ach = spmm_bytes / (spmm_ms * 1e-3) / 1e9 if spmm_ms > 0 else None
     out = {"metric": f"cells/sec for mu.tl.mofa (RNA {D_rna} genes + ATAC {args.peaks} peaks, k={K}, {iters} iterations)",
            "value": Nm / (ms_fit / 1e3), "unit": "cells/s", "ms_per_fit": ms_fit, "ms_per_iteration": ms_fit / iters,
@@ -626,12 +666,13 @@ def mofa_leg(ctx, args, box, tb, n_local, n_total, free):
 
 
 def cfg3_leg(ctx, args, free):
-    """BASELINE configs[3]: LSI k=100 on 4M cells x 500k peaks, 8 GPUs (500k cells per rank), 2 % nnz, 128 planted
-    topics (T >= k+14, SURVEY App. E); Gram / A^T U allreduces over NVLink."""
+    """BASELINE configs[3]: LSI k=100 on 2M cells x 500k peaks, 8 GPUs (250k cells per rank: 2.5e9 non-zeros, ~52 GB of
+    HBM at the peak on an 80 GB H100), 2 % nnz, 128 planted topics (T >= k+14, SURVEY App. E); Gram / A^T U
+    allreduces over NVLink."""
     import torch
     from muon_b200._synth import generate_device, make_tables
     world, rank = ctx.world, ctx.rank
-    n, D, k, dens, topics = 4_000_000 // max(world, 1) if world >= 8 else 500_000, 500_000, 100, 0.02, 128
+    n, D, k, dens, topics = 2_000_000 // max(world, 1) if world >= 8 else 250_000, 500_000, 100, 0.02, 128
     tb = make_tables(D, dens, topics, 3)
     A = generate_device(n, D, dens, tables=tb, row0=rank * n, n_total=n * world)
     ms, kern, launches, info, _ = timed_steps(ctx, lsi_step_fn(ctx, A, k, args.tol), 2, 1)

@@ -1,5 +1,5 @@
 /*
- * muon_b200.h -- C ABI of the B200-native sparse hot path of scverse/muon.
+ * muon_b200.h -- C ABI of the H100-native sparse hot path of scverse/muon.
  *
  * muon itself is pure Python and has no FFI: the reference boundary for this path is the
  * Python signature of mu.atac.pp.tfidf / mu.atac.tl.lsi / mu.tl.mofa (SURVEY.md section 8b).
@@ -129,7 +129,8 @@ int mub_csr_transpose_fill(const int64_t* indptr, const int32_t* indices, const 
 int mub_csr_transpose_fill_pairs(const int64_t* indptr, const int32_t* indices, const float* data,
                                  int64_t n_rows, int32_t n_cols, int64_t row_offset, const int64_t* t_indptr,
                                  int64_t* cursor, int32_t* t_pairs, mub_stream_t stream);
-/* fill_pairs without global atomics, for a row panel that starts on a row-block boundary: rb_count points at the
+/* fill_pairs without global atomics and in a fixed order (every transposed row lists its source rows in ascending
+ * order, so sums over it are the same on every run), for a row panel that starts on a row-block boundary: rb_count points at the
  * panel's first row block (see mub_tfidf_reduce_tiled_f32), indptr at its first row, t_indptr[n_cols+1] are the panel's
  * transposed row offsets, base is uint32 scratch [ceil(n_rows / tile height)][n_cols] (the scanned write offsets),
  * status (int32, zeroed by the caller) gets bit0 if counts and t_indptr disagree (then the result is invalid). */
@@ -204,11 +205,11 @@ int mub_mofa_loglik_f32(const float* zeta, const float* obs, int64_t n_rows, int
 int mub_knn_l2_f32(const float* X, int64_t nq, const float* Y, int64_t nc, int32_t d, int32_t ld, int32_t k,
                    int32_t* out_idx, float* out_dist, mub_stream_t stream);
 
-/* Same result (bit-identical indices and distances), tensor-core version: tcgen05 TF32 inner products in TMEM select
- * the candidates (threshold widened by the TF32 error bound so that no true neighbour is lost), an fp32 pass with
- * the arithmetic of mub_knn_l2_f32 ranks them.  d <= 128, k <= 512.  `workspace` of
+/* Same result (bit-identical indices and distances), tensor-core version: wgmma TF32 inner products (3xTF32 for
+ * d <= 64) select the candidates (threshold widened by the TF32 error bound so that no true neighbour is lost), an
+ * fp32 pass with the arithmetic of mub_knn_l2_f32 ranks them.  d <= 128, k <= 512.  `workspace` of
  * mub_knn_l2_tc_workspace_bytes(nq, nc, d) bytes; *status (zeroed by the caller) gets bit1 if some query had more than
- * ~900 points inside its error band (result then incomplete: use mub_knn_l2_f32), bit2 on an internal timeout. */
+ * ~900 points inside its error band (result then incomplete: use mub_knn_l2_f32). */
 size_t mub_knn_l2_tc_workspace_bytes(int64_t nq, int64_t nc, int32_t d);
 int mub_knn_l2_tc_f32(const float* X, int64_t nq, const float* Y, int64_t nc, int32_t d, int32_t ld, int32_t k,
                       int32_t* out_idx, float* out_dist, void* workspace, size_t workspace_bytes, int32_t* status,

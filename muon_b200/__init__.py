@@ -1,4 +1,4 @@
-"""muon_b200 -- B200-native (sm_100a) drop-in for muon's sparse hot path.
+"""muon_b200 -- H100-native (sm_90a) drop-in for muon's sparse hot path.
 
     import muon_b200 as mu
     mu.atac.pp.tfidf(adata)      # muon/_atac/preproc.py:16

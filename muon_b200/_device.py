@@ -20,7 +20,7 @@ PAD_WIDTHS = (32, 64, 128)
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise MuonB200Error("muon_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise MuonB200Error("muon_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     load()
 
 
@@ -55,8 +55,8 @@ class _timed:
 def copy_threads() -> int:
     """Host threads that fill / drain the pinned staging ring: $MUON_B200_COPY_THREADS, else half the cores this
     process may use divided by the ranks sharing the host (torchrun's LOCAL_WORLD_SIZE), clamped to [4, 16]:
-    on the benchmark host 16 threads reach 44-49 GB/s of the 55 GB/s the DMA engine delivers from pinned memory,
-    more threads are slower (profiles/staging_probe_r2.json: 48 threads 21-38 GB/s, 96 threads 10-19 GB/s)."""
+    many concurrent copy streams contend for the host's memory system, so more threads can be slower
+    (profiles/staging_probe.py measures it)."""
     env = os.environ.get("MUON_B200_COPY_THREADS")
     if env:
         return max(1, int(env))
@@ -176,9 +176,7 @@ def device_fingerprints(t: torch.Tensor, ranges) -> list:
 
 class _HostArena:
     """Recycles large host result arrays.  Fresh anonymous memory is expensive here twice over -- the first touch
-    of every page while the download is written into it and the unmapping when the array dies (measured on the
-    benchmark host, a microVM: 12 GB/s into a fresh array against the staging rate into touched memory, seconds to
-    free 24 GB) -- so blocks are kept and handed out again once NOTHING references them any more (the arrays we
+    of every page while the download is written into it and the unmapping when the array dies -- so blocks are kept and handed out again once NOTHING references them any more (the arrays we
     return are views whose ``base`` is the block, so a live result, or any view of it a caller holds, pins it).
     At most $MUON_B200_HOST_CACHE_GB (default 64) are retained; ``trim()`` returns them to the OS."""
 
@@ -530,8 +528,8 @@ class TransposedPanels:
     exceed what stays resident in L2 the gathers fall through to HBM, so the cells are cut into
     panels whose slice of Y fits in L2 and the products are accumulated panel by panel."""
 
-    # bytes of the gathered operand per panel (B200 L2: 126 MB, shared with the CSR stream)
-    L2_BUDGET = int(os.environ.get("MUON_B200_L2_BUDGET_MB", "32")) << 20
+    # bytes of the gathered operand per panel (H100 L2: 50 MB, shared with the CSR stream)
+    L2_BUDGET = int(os.environ.get("MUON_B200_L2_BUDGET_MB", "16")) << 20
 
     def __init__(self, A: DeviceCSR, pad: int = 64, side_stream: bool = False):
         n = A.shape[0]
@@ -549,10 +547,10 @@ class TransposedPanels:
             if "col_counts" in aux and list(aux["col_counts"][0]) == cb:
                 cc = aux["col_counts"][1]
                 counts = [cc[i * per:(i + 1) * per].sum(0, dtype=torch.int64) for i in range(n_panels)]
-                # opt-in: the atomic-free tiled fill is correct but SLOWER at configs[1] (180 ms against 105 ms:
-                # each (row block, column) writes a ~120-byte run at its own time, so L2 merges less than under the
-                # row-ordered atomic-cursor fill) -- profiles/README.md, negative results
-                if os.environ.get("MUON_B200_FILL_TILED", "0") == "1" and not side_stream:
+                # the tiled fill lists every transposed row in ascending cell order, so A^T Y sums in the same
+                # order on every run (the atomic-cursor fill's order follows slot claims); MUON_B200_FILL_TILED=0
+                # selects the atomic-cursor fill
+                if os.environ.get("MUON_B200_FILL_TILED", "1") == "1" and not side_stream:
                     rb = aux.get("rb_counts")
         else:
             bounds = [round(i * n / n_panels) for i in range(n_panels + 1)]
@@ -743,7 +741,7 @@ def gram(Y: torch.Tensor, l: Optional[int] = None, weights: Optional[torch.Tenso
 # muon/_atac/preproc.py:86-129), with the device work hidden under the transfers:
 #   upload    row block b+1 is staged/uploaded on a copy stream while the reduce kernel runs on block b
 #             (int64 indices -> int32 and float32 counts -> uint8 inside the staging copy)
-#   download  one apply launch over all rows (20 ms), then one staged download into a recycled host buffer
+#   download  one apply launch over all rows, then one staged download into a recycled host buffer
 # Fingerprints of what crossed the bus are taken on the device copies afterwards (csrc/staging.cu).
 _BLOCK_NNZ = int(os.environ.get("MUON_B200_BLOCK_NNZ", str(192 << 20)))
 
@@ -832,7 +830,7 @@ def tfidf_from_host(X, log_tf=True, log_idf=True, log_tfidf=False, scale_factor=
     with _timed("alloc_out_s"):
         out_h = _ARENA.empty(nnz, np.float32)
 
-    # apply over all rows (20 ms at configs[1]), then ONE download call: every d2h call drains its pipeline before it
+    # apply over all rows, then ONE download call: every d2h call drains its pipeline before it
     # returns, so downloading block by block (to overlap the apply kernels) cost more in bubbles than it hid
     if blocks:
         call("mub_tfidf_apply_f32", ptr(indptr), ptr(indices), ptr(data), ptr(data), n, d, ptr(row_sum), ptr(idf),
@@ -840,7 +838,7 @@ def tfidf_from_host(X, log_tf=True, log_idf=True, log_tfidf=False, scale_factor=
         side.wait_event(main.record_event())
         st.d2h(data, out_h, stream=side)
     main.wait_stream(side)
-    # fingerprints of what crossed the bus, taken on the device copies (HBM-bound: ~10 ms per 24 GB) instead of
+    # fingerprints of what crossed the bus, taken on the device copies (HBM-bound) instead of
     # inside the host-side staging loops
     ranges = [(k0, k1) for (_, _, k0, k1) in blocks]
     fp_idx = device_fingerprints(indices, ranges)
@@ -960,7 +958,7 @@ def knn_l2(X: torch.Tensor, k: int, Y: Optional[torch.Tensor] = None, algo: Opti
     Returns (indices int32 [n x k], distances float32 [n x k]), ascending, ties by lower index.  Groundwork for
     the WNN row (reference muon/_core/preproc.py:520-528).
 
-    algo: "simt" (fp32 CUDA-core kernel), "tc" (tcgen05 TF32 candidate pass + fp32 re-rank, same result; falls back
+    algo: "simt" (fp32 CUDA-core kernel), "tc" (wgmma TF32 candidate pass + fp32 re-rank, same result; falls back
     to "simt" -- another GPU kernel, not the host -- if a query has too many points inside the TF32 error band)
     or None = $MUON_B200_KNN, default "tc"."""
     require_cuda()
@@ -982,8 +980,6 @@ def knn_l2(X: torch.Tensor, k: int, Y: Optional[torch.Tensor] = None, algo: Opti
         call("mub_knn_l2_tc_f32", ptr(X), nq, ptr(Y), Y.shape[0], d, d, k, ptr(idx), ptr(dist), ptr(ws), nbytes,
              ptr(status), stream_ptr())
         st = int(status[0])
-        if st & 4:
-            raise MuonB200Error("knn_l2(algo='tc'): tcgen05 commit never arrived (internal error)")
         if st == 0:
             return idx, dist
         # st & 2: error band too crowded for some query -> exact SIMT kernel below

@@ -2,7 +2,7 @@
 
 The reference computes ``svds(adata.X, k)`` (muon/_atac/tools.py:53): ARPACK ``eigsh`` on the
 implicit X^T X, one vector at a time -- 300-900 single-vector passes over the matrix for
-k=50 (SURVEY section 6).  On a B200 every pass streams the whole CSR from HBM, so the design
+k=50 (SURVEY section 6).  On an H100 every pass streams the whole CSR from HBM, so the design
 goal is *few, wide* passes: a block of ``b`` vectors (b = padded kernel width, 64 for k=50)
 per pass and a Krylov method that converges in a handful of block steps.
 
@@ -92,8 +92,8 @@ class CsrOperator:
                 w.wait()
             return W
 
-    # measured (profiles/README.md, multi-GPU): 4 blocks hide a ~0.3 ms allreduce but cost ~25 ms per step in smaller,
-    # less efficient SpMM launches, so the default is one block (the overlapped path stays available and tested)
+    # several blocks overlap the allreduce with the product but split the SpMM into smaller, less efficient
+    # launches, and the allreduce of a d x P block is short, so the default is one block (the overlapped path stays available and tested)
     AR_CHUNKS = int(os.environ.get("MUON_B200_AR_CHUNKS", "1"))
 
     def residual_sample(self, Uk, Vk, sig):

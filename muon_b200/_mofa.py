@@ -623,7 +623,7 @@ def mofa(
     for flag, name in ((svi_mode, "svi_mode"), (smooth_covariate, "smooth_covariate"),
                        (spikeslab_factors, "spikeslab_factors"), (use_raw, "use_raw")):
         if flag:
-            raise NotImplementedError(f"mofa(..., {name}=...) is not supported by the B200 path yet")
+            raise NotImplementedError(f"mofa(..., {name}=...) is not supported by the CUDA path yet")
     lik = likelihoods
     if lik is not None:
         lik = [lik] * len(mdata.mod) if isinstance(lik, str) else list(lik)

@@ -19,11 +19,11 @@ int sm_count() {
     // thread-local cache keyed by device id: no global mutable state shared across threads
     static thread_local int cached_dev = -1, cached_sms = 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev != cached_dev) {
         int n = 0;
         if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-            n = 148;
+            n = 132;
         cached_dev = dev;
         cached_sms = n;
     }

@@ -13,7 +13,7 @@
 // At the end every list is sorted ascending by (distance, index) and the distances are square-rooted.
 //
 // fp32 SIMT first (distances accurate to fp32 rounding, self-distance exactly 0, ties resolved by index);
-// a tcgen05 TF32 candidate pass + fp32 re-rank is the round-2 upgrade.
+// knn_tc.cu adds a tensor-core (wgmma TF32) candidate pass + fp32 re-rank with the same result.
 #include <float.h>
 
 #include "common.cuh"

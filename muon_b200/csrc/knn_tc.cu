@@ -1,16 +1,16 @@
-// Exact k-nearest-neighbour search, tensor-core candidate pass + fp32 re-rank (tcgen05 / TMEM, sm_100a).
+// Exact k-nearest-neighbour search, tensor-core candidate pass + fp32 re-rank (wgmma TF32, sm_90a).
 //
 // Same contract as knn.cu (mub_knn_l2_f32): the k nearest rows of Y for every row of X in Euclidean distance,
 // ascending, ties by lower index, distances bit-identical to the SIMT kernel.  The n x n inner-product matrix is
-// the one GEMM-shaped operation of the WNN row (reference muon/_core/preproc.py:520-528), so it runs on the 5th-gen
-// tensor cores:
+// the one GEMM-shaped operation of the WNN row (reference muon/_core/preproc.py:520-528), so it runs on the
+// Hopper tensor cores:
 //
-//   pass 1  knn_tc_candidates_kernel: one CTA owns 128 queries (M = 128 = the TMEM lanes).  Candidate tiles of 128
-//           points are written to shared memory in the canonical no-swizzle K-major layout (8-row x 16-byte core
-//           matrices, SBO 128 B, LBO 2048 B; validated by experimental/umma_probe.cu), one elected thread issues
-//           ceil(d/8) tcgen05.mma.kind::tf32 instructions that accumulate S = Q C^T in 128 TMEM columns and commits
-//           to an mbarrier; the 128 threads then read their own row of S with tcgen05.ld (thread t = TMEM lane t),
-//           form a(q,c) = |c|^2 - 2 S and keep every candidate with a <= tau_q in a per-query buffer.
+//   pass 1  knn_tc_candidates_kernel: one CTA (one warpgroup of 128 threads) owns 128 queries.  Candidate tiles of
+//           128 points are written to shared memory in the canonical no-swizzle K-major layout (8-row x 16-byte core
+//           matrices, SBO 128 B between 8-row groups, LBO 2048 B between K chunks); the warpgroup issues
+//           2 x ceil(d/8) wgmma.mma_async m64n128k8 TF32 instructions (query rows 0-63 and 64-127) that accumulate
+//           S = Q C^T in registers, waits for them, and stages S through shared memory so that thread t holds row t;
+//           each thread then forms a(q,c) = |c|^2 - 2 S and keeps every candidate with a <= tau_q in a per-query buffer.
 //           TF32 truncates the inputs to 10 mantissa bits, so a() carries an error of at most 2^-8 |q||c| -- too
 //           coarse for concentrated distance distributions, so for d <= 64 the operands are split 3xTF32
 //           (big + small parts along a tripled K axis, see knn_tc_pack_kernel) and the error drops to ~5e-5 |q||c|.
@@ -24,8 +24,8 @@
 //
 // Operands are packed once per call (knn_tc_pack_kernel) into per-tile blocks that already have the shared-memory
 // layout, so that staging a tile is one contiguous, fully coalesced copy (and can become a single 1-D TMA bulk copy).
-// First version: single-stage (load -> MMA -> epilogue in sequence; the CTAs co-resident on an SM overlap each
-// other), plain global->shared copies.  Every mbarrier wait is bounded; a timeout is reported through `status`.
+// Single-stage (load -> MMA -> epilogue in sequence; the CTAs co-resident on an SM overlap each other), plain
+// global->shared copies.
 #include <float.h>
 #include <math.h>
 
@@ -33,21 +33,74 @@
 
 namespace mub {
 
-constexpr int kTcM = 128;        // queries per CTA tile = TMEM lanes
-constexpr int kTcN = 128;        // candidates per MMA tile = TMEM columns
+constexpr int kTcM = 128;        // queries per CTA tile (two m64 row halves)
+constexpr int kTcN = 128;        // candidates per MMA tile (wgmma N)
 constexpr int kTcCap = 1024;     // candidate buffer entries per query
-constexpr int kTcThreads = 128;
+constexpr int kTcThreads = 128;  // one warpgroup
+constexpr int kTcSLd = kTcN + 1; // row stride (floats) of the staged score tile: thread t reads row t without bank conflicts
 
 __device__ __forceinline__ uint32_t tc_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// shared-memory matrix descriptor, K-major, no swizzle (cute/arch/mma_sm100_desc.hpp bit layout)
-__device__ __forceinline__ uint64_t tc_umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// wgmma shared-memory matrix descriptor, K-major, no swizzle (layout type 0 in bits 62-63, base offset 0):
+// start address, leading-dimension byte offset (between core matrices along K), stride-dimension byte offset
+// (between 8-row groups along M / N), all in 16-byte units
+__device__ __forceinline__ uint64_t tc_wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= 1ull << 46;                                    // descriptor version 1 (Blackwell)
     return d;
+}
+
+// D[64 x 128] (+)= A[64 x 8] . B[128 x 8]^T in TF32, fp32 accumulators in the warpgroup's registers.  Fragment:
+// thread t (warp w = t/32, lane l) holds d[4j + 2i + c] = D[16w + l/4 + 8i][8j + 2(l%4) + c].
+__device__ __forceinline__ void tc_wgmma_m64n128k8(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+        "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
+}
+
+// scores of one 128 x 128 tile pair, S = Q C^T -> shared memory sS[row * kTcSLd + col].  sS aliases sC: every wgmma of
+// the tile has completed (and every thread passed a barrier) before the first score is stored.
+__device__ __forceinline__ void tc_scores(const unsigned char* sQ, const unsigned char* sC, float* sS, int Kp, int tid) {
+    float acc[2][64];                                           // no initialisation: the first k-step has scale-d = 0
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    const uint32_t lbo_q = kTcM * 16, lbo_c = kTcN * 16, sbo = 128;
+    for (int ks = 0; ks < Kp / 8; ++ks) {                       // k8 = two 16-byte K chunks
+        const uint64_t db = tc_wgmma_desc(tc_smem_u32(sC) + (uint32_t)(2 * ks) * lbo_c, lbo_c, sbo);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint64_t da = tc_wgmma_desc(tc_smem_u32(sQ) + (uint32_t)(2 * ks) * lbo_q + (uint32_t)h * 64 * 16, lbo_q, sbo);
+            tc_wgmma_m64n128k8(acc[h], da, db, ks > 0 ? 1u : 0u);
+        }
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    __syncthreads();
+    const int w = tid >> 5, l = tid & 31;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < kTcN / 8; ++j)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                float* dst = sS + (size_t)(h * 64 + 16 * w + (l >> 2) + 8 * i) * kTcSLd + 8 * j + 2 * (l & 3);
+                dst[0] = acc[h][4 * j + 2 * i];
+                dst[1] = acc[h][4 * j + 2 * i + 1];
+            }
+    __syncthreads();
 }
 
 // monotone map float -> uint32 (order preserving, total on non-NaN)
@@ -176,44 +229,25 @@ knn_tc_candidates_kernel(const float4* __restrict__ Xpk, const float* __restrict
                          int32_t* __restrict__ ibuf, int32_t* __restrict__ cand, int32_t* __restrict__ cand_cnt,
                          int32_t* __restrict__ status) {
     extern __shared__ __align__(1024) unsigned char smem[];
-    __shared__ __align__(8) uint64_t bar;
-    __shared__ uint32_t tmem_base_s;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     const int chunks = Kp / 4;                                  // 16-byte K chunks (4 tf32 values)
     unsigned char* sQ = smem;                                   // [chunks][128][16 B]
-    unsigned char* sC = smem + (size_t)chunks * kTcM * 16;      // [chunks][128][16 B]
-    float* sCn = reinterpret_cast<float*>(sC + (size_t)chunks * kTcN * 16);   // [2][128] candidate norms
+    unsigned char* sC = smem + (size_t)chunks * kTcM * 16;      // [chunks][128][16 B], then the score tile in its place
+    float* sS = reinterpret_cast<float*>(sC);                   // [128][kTcSLd]
+    const size_t c_bytes = (size_t)chunks * kTcN * 16, s_bytes = sizeof(float) * kTcM * kTcSLd;
+    float* sCn = reinterpret_cast<float*>(sC + (c_bytes > s_bytes ? c_bytes : s_bytes));   // [2][128] candidate norms
     int32_t* hist = reinterpret_cast<int32_t*>(sCn + 2 * kTcN);               // [16][128] radix-select counters
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&tmem_base_s)), "r"(kTcN));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tc_smem_u32(&bar)));
-        asm volatile("fence.mbarrier_init.release.cluster;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    const uint32_t tmem_base = tmem_base_s;
 
     float* kb = kbuf + (size_t)blockIdx.x * kTcCap * kTcM;
     int32_t* ib = ibuf + (size_t)blockIdx.x * kTcCap * kTcM;
     const float cmax = sqrtf(__uint_as_float(*ymax_bits));
-    uint32_t idesc = 0;
-    idesc |= 1u << 4;                                           // accumulator f32
-    idesc |= 2u << 7;                                           // A = tf32
-    idesc |= 2u << 10;                                          // B = tf32
-    idesc |= (uint32_t)(kTcN >> 3) << 17;
-    idesc |= (uint32_t)(kTcM >> 4) << 24;
 
     const int64_t n_qt = (nq + kTcM - 1) / kTcM;
-    uint32_t it = 0;                                            // MMA batches issued so far (mbarrier phase = it & 1)
-    bool dead = false;
-    for (int64_t qt = blockIdx.x; qt < n_qt && !dead; qt += gridDim.x) {
+    uint32_t it = 0;                                            // candidate tiles processed so far (norm buffer = it & 1)
+    for (int64_t qt = blockIdx.x; qt < n_qt; qt += gridDim.x) {
         const int64_t row = qt * kTcM + tid;
         const bool live = row < nq;
+        __syncthreads();                                        // the previous query tile's wgmma reads of sQ are done
         {   // the packed tile already has the shared-memory layout: contiguous copy
             const float4* src = Xpk + (size_t)qt * chunks * kTcM;
             float4* dst = reinterpret_cast<float4*>(sQ);
@@ -240,6 +274,7 @@ knn_tc_candidates_kernel(const float4* __restrict__ Xpk, const float* __restrict
             }
             const int64_t crow = c0 + tid;
             const bool cl = crow < nc;
+            __syncthreads();                                    // every thread has read the previous score tile (sS = sC)
             {
                 const float4* src = Ypk + (size_t)(c0 / kTcN) * chunks * kTcN;
                 float4* dst = reinterpret_cast<float4*>(sC);
@@ -248,51 +283,14 @@ knn_tc_candidates_kernel(const float4* __restrict__ Xpk, const float* __restrict
             }
             float* cn = sCn + (it & 1) * kTcN;
             cn[tid] = cl ? ynorm[crow] : INFINITY;
-            asm volatile("fence.proxy.async.shared::cta;");     // generic stores -> async proxy (tensor core reads)
-            asm volatile("tcgen05.fence::before_thread_sync;"); // orders the previous tile's tcgen05.ld before the barrier
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> async proxy (wgmma reads)
             __syncthreads();
-            asm volatile("tcgen05.fence::after_thread_sync;");
-            if (tid == 0) {
-                const uint32_t lbo = kTcM * 16, sbo = 128;
-                for (int ks = 0; ks < Kp / 8; ++ks) {
-                    const uint64_t da = tc_umma_desc(tc_smem_u32(sQ) + (uint32_t)(2 * ks) * kTcM * 16, lbo, sbo);
-                    const uint64_t db = tc_umma_desc(tc_smem_u32(sC) + (uint32_t)(2 * ks) * kTcN * 16, lbo, sbo);
-                    const uint32_t acc = ks > 0 ? 1u : 0u;
-                    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_base),
-                                 "l"(da), "l"(db), "r"(idesc), "r"(acc));
-                }
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tc_smem_u32(&bar))
-                             : "memory");
-            }
-            uint32_t done = 0;
-            for (int spin = 0; spin < (1 << 22) && !done; ++spin) {
-                asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                             : "=r"(done)
-                             : "r"(tc_smem_u32(&bar)), "r"(it & 1u)
-                             : "memory");
-            }
-            if (__syncthreads_or(done ? 0 : 1)) {               // the commit never arrived: give up, report
-                dead = true;
-                break;
-            }
-            asm volatile("tcgen05.fence::after_thread_sync;");
+            tc_scores(sQ, sC, sS, Kp, tid);
+            const float* srow = sS + (size_t)tid * kTcSLd;
             for (int cc = 0; cc < kTcN; cc += 32) {
-                uint32_t r[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)cc;
-                __syncwarp();                                   // tcgen05.ld is .sync.aligned: reconverge after the appends
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-                    "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-                    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                      "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                      "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                      "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 #pragma unroll
                 for (int j = 0; j < 32; ++j) {
-                    const float a = fmaf(-2.f, __uint_as_float(r[j]), cn[cc + j]);
+                    const float a = fmaf(-2.f, srow[cc + j], cn[cc + j]);
                     if (a <= tau && c0 + cc + j < nc) {
                         if (cnt < kTcCap) {
                             kb[(size_t)cnt * kTcM + tid] = a;
@@ -305,19 +303,12 @@ knn_tc_candidates_kernel(const float4* __restrict__ Xpk, const float* __restrict
                 }
             }
         }
-        if (dead) break;
         tc_compact(kb, ib, hist, tid, k, slack, cnt, tau);      // final trim
         if (live) {
             cand_cnt[row] = cnt;
             for (int i = 0; i < cnt; ++i) cand[(size_t)row * kTcCap + i] = ib[(size_t)i * kTcM + tid];
             if (overflow) atomicOr(status, 2);
         }
-    }
-    if (dead && tid == 0) atomicOr(status, 4);
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTcN));
     }
 }
 
@@ -453,8 +444,9 @@ int mub_knn_l2_tc_f32(const float* X, int64_t nq, const float* Y, int64_t nc, in
     // K <= 192 terms (<= 2^-23 each) -> |da| <= 4.6e-5 |q||c|.  tau needs twice the bound; the plain variant doubles it
     // once more for safety.
     const float slack_rel = L.split ? 1.2e-4f : 4.f * 0.00390625f;
-    const size_t smem = (size_t)(Ktot / 4) * (mub::kTcM + mub::kTcN) * 16 + 2 * mub::kTcN * sizeof(float) +
-                        16 * mub::kTcM * sizeof(int32_t);
+    const size_t c_bytes = (size_t)(Ktot / 4) * mub::kTcN * 16, s_bytes = sizeof(float) * mub::kTcM * mub::kTcSLd;
+    const size_t smem = (size_t)(Ktot / 4) * mub::kTcM * 16 + (c_bytes > s_bytes ? c_bytes : s_bytes) +
+                        2 * mub::kTcN * sizeof(float) + 16 * mub::kTcM * sizeof(int32_t);
     e = cudaFuncSetAttribute(mub::knn_tc_candidates_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
         mub::set_error("knn_l2_tc: %zu B of shared memory: %s", smem, cudaGetErrorString(e));

@@ -1,4 +1,4 @@
-// K5 -- MOFA+ coordinate-ascent row updates for sm_100a (gaussian views, spike-and-slab weights).
+// K5 -- MOFA+ coordinate-ascent row updates for sm_90a (gaussian views, spike-and-slab weights).
 //
 // The reference hands densified modalities to mofapy2 (muon/_core/tools.py:117-141,583-585),
 // whose per-iteration cost is dense N x D_m GEMMs and elementwise N x D_m passes.  Here the data

@@ -1,4 +1,4 @@
-// K2/K3 -- CSR x dense SpMM  C[n x P] (+)= A[n x d] * B[d x P]  for sm_100a, P in {32,64,128}.
+// K2/K3 -- CSR x dense SpMM  C[n x P] (+)= A[n x d] * B[d x P]  for sm_90a, P in {32,64,128}.
 //
 // Replaces the per-Lanczos-step csr_matvec/csc_matvec pair that ARPACK drives inside
 // scipy.sparse.linalg.svds (scipy _svds.py:428-460, called at muon/_atac/tools.py:53) by a
@@ -162,19 +162,14 @@ __device__ __forceinline__ void spmm_row_h(const int32_t* __restrict__ indices, 
     constexpr int STEPS = 32 / G;   // gathers per 32-nnz segment
     const int sub = lane % LPN, grp = lane / LPN;
     const __half* Bl = B + sub * 8;
-    // accumulators as four packed float2 (64-bit registers): Blackwell's fma.rn.f32x2 retires two fp32 FMAs per
-    // issue slot, and with the half operand this kernel is bound by issue slots (ncu: 65 % issue-active), not by L2
-    unsigned long long acc2[4] = {0ull, 0ull, 0ull, 0ull};
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     auto fma8 = [&](float v, const uint4& q) {
-        unsigned long long vv2;
-        asm("mov.b64 %0, {%1, %1};" : "=l"(vv2) : "f"(v));
         const unsigned w[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-            unsigned long long b2;
-            asm("mov.b64 %0, {%1, %2};" : "=l"(b2) : "f"(f.x), "f"(f.y));
-            asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[i]) : "l"(vv2), "l"(b2));
+            acc[2 * i] = fmaf(v, f.x, acc[2 * i]);
+            acc[2 * i + 1] = fmaf(v, f.y, acc[2 * i + 1]);
         }
     };
     int64_t base = start;
@@ -215,9 +210,6 @@ __device__ __forceinline__ void spmm_row_h(const int32_t* __restrict__ indices, 
             if (src < cnt) fma8(vt, ld_gather_u4(Bl + (size_t)cc * P));
         }
     }
-    float acc[8];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) asm("mov.b64 {%0, %1}, %2;" : "=f"(acc[2 * i]), "=f"(acc[2 * i + 1]) : "l"(acc2[i]));
 #pragma unroll
     for (int off = LPN; off < 32; off <<= 1) {
 #pragma unroll
@@ -237,8 +229,6 @@ __device__ __forceinline__ void spmm_row_h(const int32_t* __restrict__ indices, 
     }
 }
 
-// (forcing 4 CTAs/SM -- 64 registers instead of 76 -- was measured: 52.3 ms per pass against 51.7, the spills cost what
-// the occupancy gains; profiles/README.md)
 template <int P, bool PAIRS>
 __global__ void __launch_bounds__(kSpmmThreads)
 spmm_csr_rowwarp_h_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,

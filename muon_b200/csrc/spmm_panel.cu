@@ -1,7 +1,7 @@
 // K2 v2 -- CSR x dense SpMM with the dense operand staged through shared memory by TMA.
 //
-// The v1 row-warp kernel (spmm.cu) gathers 4P bytes of B per non-zero straight from L2; ncu shows
-// it pinned at ~80 % of L2 bandwidth with a 1 % L1 hit rate.  Here a persistent CTA owns a block
+// The v1 row-warp kernel (spmm.cu) gathers 4P bytes of B per non-zero straight from L2, with almost
+// no L1 reuse.  Here a persistent CTA owns a block
 // of R = 32*warps rows and sweeps the COLUMN axis in panels: panel p of B (panel_cols x P floats,
 // contiguous in row-major B) is copied into shared memory by one cp.async.bulk (TMA) per panel,
 // double-buffered behind mbarriers, and every row of the block consumes its non-zeros whose

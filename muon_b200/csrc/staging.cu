@@ -273,8 +273,7 @@ int mub_stager_destroy(void* handle) {
 // The array is cut into one contiguous slab per worker thread; every worker converts its slab piece by piece into
 // its two private pinned sub-buffers and enqueues the DMA of each piece on `stream` itself (the runtime API is
 // thread-safe; copies of different workers interleave on the stream).  One wake-up of the pool per CALL -- an
-// earlier version synchronised the pool once per 64 MB chunk and stopped scaling at 16 threads
-// (profiles/staging_probe_r2.json).  Returns when the last piece is enqueued.
+// earlier version synchronised the pool once per 64 MB chunk.  Returns when the last piece is enqueued.
 int mub_stager_h2d(void* handle, const void* src_h, void* dst, size_t n_elems, int32_t src_elem_bytes, int32_t narrow,
                    uint64_t* hash_h, int32_t* overflow_h, mub_stream_t stream) {
     using namespace mub;

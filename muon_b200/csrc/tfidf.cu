@@ -1,4 +1,4 @@
-// K1 -- fused CSR TF-IDF for sm_100a (reference arithmetic: muon/_atac/preproc.py:92-119).
+// K1 -- fused CSR TF-IDF for sm_90a (reference arithmetic: muon/_atac/preproc.py:92-119).
 //
 // Two streaming passes over the CSR arrays, both HBM-bound:
 //   reduce : reads indices+values (8 B/nnz fp32), warp-shuffle row sums, column sums by
@@ -85,7 +85,7 @@ tfidf_reduce_kernel(const int64_t* __restrict__ indptr, const int32_t* __restric
 
 // ---- tiled reduce (fp32, rows with sorted column indices) -----------------------------------------------
 // The kernel above issues one global RED per non-zero into the D-vector of column sums: 6e9 atomics at
-// BASELINE configs[1], and it is their rate (not HBM) that bounds it (31 ms, 18 % of DRAM bandwidth).  Here a CTA
+// BASELINE configs[1], and it is their rate (not HBM) that bounds it.  Here a CTA
 // owns a block of kTileRows rows and sweeps the column range tile by tile (kTileCols columns): the tile's
 // column sums AND entry counts live in shared memory, every non-zero costs two shared-memory atomics, and the
 // tile is flushed to global memory once per (row block, tile) -- ~30x fewer global atomics.  Rows are sorted, so

@@ -103,16 +103,21 @@ transpose_fill_pairs_kernel(const int64_t* __restrict__ indptr, const int32_t* _
     }
 }
 
-// ---- tiled fill: no global atomics ------------------------------------------------------------------------
-// The atomic-cursor fill above spends one global ATOM (with return) plus one scattered 8-byte store per non-zero
-// and is bound by that queue (ncu: lg_throttle 289, issue-active 2 %).  When the TF-IDF reduce pass has left the
-// entry count of every (512-row block, column) behind (tfidf.cu, rb_count), the write offset of block b in
-// column c is  t_indptr[c] + sum of the counts of the panel's earlier blocks  -- a column-wise scan -- and a CTA
-// that owns block b only has to hand out consecutive slots INSIDE its own range: per-column cursors in shared
-// memory, tile by tile over the columns, exactly the sweep of tfidf_reduce_tiled_kernel.
-constexpr int kFillTileCols = 12288;   // 48 KB of cursors
+// ---- tiled fill: no global atomics, deterministic ------------------------------------------------------------
+// The atomic-cursor fill above spends one global ATOM (with return) plus one scattered 8-byte store per non-zero,
+// and the order in which slots are claimed -- hence the order of the entries inside a transposed row, hence the fp32
+// summation order of every A^T Y product -- changes from run to run.  When the TF-IDF reduce pass has left the
+// entry count of every (512-row block, column) behind (tfidf.cu, rb_count), the write offset of block b in column c
+// is  t_indptr[c] + sum of the counts of the panel's earlier blocks  -- a column-wise scan.  Inside its block a CTA
+// sweeps the columns tile by tile; warp w owns the 32 consecutive rows [32w, 32w + 32) and walks them in order.
+// Per tile it first counts its entries per column (the columns of one row are distinct, so the lanes never collide),
+// the counts are scanned over the warps in warp order, and a second walk writes every entry at the next slot of its
+// (warp, column) cursor.  Every transposed row therefore lists its cells in ascending order, on every run.
+constexpr int kFillTileCols = 2048;    // 16 warps x 2048 columns x 4 B = 128 KB of per-warp cursors
 constexpr int kFillRows = 512;         // must equal the reduce kernel's block height (mub_tfidf_tile_rows)
 constexpr int kFillThreads = 512;
+constexpr int kFillWarps = kFillThreads / 32;
+constexpr int kFillRowsPerWarp = kFillRows / kFillWarps;
 
 // base[b][c] = t_indptr[c] + sum_{b' < b} count[b'][c] for the blocks of one panel (one thread per column)
 __global__ void __launch_bounds__(256)
@@ -128,57 +133,69 @@ transpose_scan_blocks_kernel(const uint16_t* __restrict__ rb_count, int32_t n_co
     if (run != (unsigned long long)t_indptr[c + 1] || run > 0xffffffffull) atomicOr(status, 1);   // counts and indptr disagree
 }
 
-__global__ void __launch_bounds__(kFillThreads, 2)
+__global__ void __launch_bounds__(kFillThreads, 1)
 transpose_fill_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
                             const float* __restrict__ data, int64_t n_rows, int32_t n_cols,
                             const uint32_t* __restrict__ base, int2* __restrict__ t_pairs) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    unsigned* cursor = reinterpret_cast<unsigned*>(smem_raw);
-    int* cur = reinterpret_cast<int*>(smem_raw + sizeof(unsigned) * kFillTileCols);
+    uint32_t* wcur = reinterpret_cast<uint32_t*>(smem_raw);                        // [kFillWarps][kFillTileCols]
+    int* cur = reinterpret_cast<int*>(wcur + kFillWarps * kFillTileCols);           // [kFillRows] entries done per row
+    int* ntile = cur + kFillRows;                                                   // [kFillRows] entries in this tile
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    constexpr int kWarps = kFillThreads / 32;
     const int64_t r0 = (int64_t)blockIdx.x * kFillRows;
     const int rows_here = (int)((n_rows - r0) < kFillRows ? (n_rows - r0) : kFillRows);
+    const int my_r0 = warp * kFillRowsPerWarp;
+    const int my_r1 = (my_r0 + kFillRowsPerWarp < rows_here) ? my_r0 + kFillRowsPerWarp : rows_here;
+    uint32_t* my_cur = wcur + warp * kFillTileCols;
     for (int r = threadIdx.x; r < kFillRows; r += kFillThreads) cur[r] = 0;
     const uint32_t* my_base = base + (size_t)blockIdx.x * n_cols;
     const int n_tiles = (n_cols + kFillTileCols - 1) / kFillTileCols;
     for (int t = 0; t < n_tiles; ++t) {
         const int c_lo = t * kFillTileCols;
         const int c_hi = (c_lo + kFillTileCols < n_cols) ? c_lo + kFillTileCols : n_cols;
-        for (int j = threadIdx.x; j < c_hi - c_lo; j += kFillThreads) cursor[j] = my_base[c_lo + j];
+        for (int j = threadIdx.x; j < kFillWarps * kFillTileCols; j += kFillThreads) wcur[j] = 0;
         __syncthreads();
-        for (int r = warp; r < rows_here; r += kWarps) {
-            const int64_t s0 = __ldg(indptr + r0 + r), e = __ldg(indptr + r0 + r + 1);
-            int64_t k = s0 + cur[r];
-            const int row_local = (int)(r0 + r);
+        // walk 1: entries per (warp, column) of this tile, and per row the number of its entries inside the tile
+        for (int r = my_r0; r < my_r1; ++r) {
+            const int64_t e = __ldg(indptr + r0 + r + 1);
+            const int64_t k0 = __ldg(indptr + r0 + r) + cur[r];
+            int64_t k = k0;
             for (;;) {
-                const int64_t k0 = k + lane, k1 = k0 + 32, k2 = k0 + 64;
-                const int c0 = k0 < e ? ld_stream(indices + k0) : 0x7fffffff;
-                const int c1 = k1 < e ? ld_stream(indices + k1) : 0x7fffffff;
-                const int c2 = k2 < e ? ld_stream(indices + k2) : 0x7fffffff;
-                const float v0 = k0 < e ? ld_stream(data + k0) : 0.f;
-                const float v1 = k1 < e ? ld_stream(data + k1) : 0.f;
-                const float v2 = k2 < e ? ld_stream(data + k2) : 0.f;
-                int taken = 0;
-                bool stop = false;
+                const int c = k + lane < e ? ld_stream(indices + k + lane) : 0x7fffffff;
+                const bool in = c < c_hi;                  // sorted row: the entries of this tile come first
+                const int n_in = __popc(__ballot_sync(0xffffffffu, in));
+                if (in && c >= c_lo) my_cur[c - c_lo] += 1;
+                k += n_in;
+                if (n_in < 32) break;
+            }
+            if (lane == 0) ntile[r] = (int)(k - k0);
+        }
+        __syncthreads();
+        // exclusive scan over the warps, in warp (= row) order, from the block's write offset of each column
+        for (int j = threadIdx.x; j < c_hi - c_lo; j += kFillThreads) {
+            uint32_t run = my_base[c_lo + j];
 #pragma unroll
-                for (int u = 0; u < 3; ++u) {
-                    const int c = u == 0 ? c0 : (u == 1 ? c1 : c2);
-                    const float v = u == 0 ? v0 : (u == 1 ? v1 : v2);
-                    const bool in = !stop && c < c_hi;
-                    const int n_in = __popc(__ballot_sync(0xffffffffu, in));
-                    if (in && c >= c_lo) {
-                        const unsigned slot = atomicAdd(&cursor[c - c_lo], 1u);
-                        t_pairs[slot] = make_int2(row_local, __float_as_int(v));
-                    }
-                    taken += n_in;
-                    if (n_in < 32) stop = true;
+            for (int w = 0; w < kFillWarps; ++w) {
+                const uint32_t cnt = wcur[w * kFillTileCols + j];
+                wcur[w * kFillTileCols + j] = run;
+                run += cnt;
+            }
+        }
+        __syncthreads();
+        // walk 2: rows in order, each entry at the next slot of its (warp, column) cursor
+        for (int r = my_r0; r < my_r1; ++r) {
+            const int64_t k0 = __ldg(indptr + r0 + r) + cur[r];
+            const int n = ntile[r];
+            for (int i = lane; i < n; i += 32) {
+                const int c = ld_stream(indices + k0 + i);
+                const float v = ld_stream(data + k0 + i);
+                if (c >= c_lo) {
+                    const uint32_t slot = my_cur[c - c_lo]++;
+                    t_pairs[slot] = make_int2((int)(r0 + r), __float_as_int(v));
                 }
-                k += taken;
-                if (stop || k >= e) break;
             }
             __syncwarp();
-            if (lane == 0) cur[r] = (int)(k - s0);
+            if (lane == 0) cur[r] += n;
         }
         __syncthreads();
     }
@@ -325,8 +342,12 @@ extern "C" int mub_csr_transpose_fill_tiled(const int64_t* indptr, const int32_t
     const int64_t n_blocks = (n_rows + mub::kFillRows - 1) / mub::kFillRows;
     MUB_REQUIRE(n_blocks < (1ll << 31), "transpose_fill_tiled: too many rows");
     mub::transpose_scan_blocks_kernel<<<(n_cols + 255) / 256, 256, 0, s>>>(rb_count, n_cols, n_blocks, t_indptr, base, status);
-    const size_t smem = sizeof(unsigned) * mub::kFillTileCols + sizeof(int) * mub::kFillRows;
-    cudaFuncSetAttribute(mub::transpose_fill_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const size_t smem = sizeof(uint32_t) * mub::kFillWarps * mub::kFillTileCols + 2 * sizeof(int) * mub::kFillRows;
+    cudaError_t e = cudaFuncSetAttribute(mub::transpose_fill_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) {
+        mub::set_error("transpose_fill_tiled: %zu B of shared memory: %s", smem, cudaGetErrorString(e));
+        return -2;
+    }
     mub::transpose_fill_tiled_kernel<<<(int)n_blocks, mub::kFillThreads, smem, s>>>(indptr, indices, data, n_rows, n_cols, base,
                                                                                   (int2*)t_pairs);
     return mub::check_launch("transpose_fill_tiled");

@@ -145,7 +145,7 @@ def neighbors(
     else:
         modalities = list(neighbor_keys.keys())
     if metric != "euclidean":
-        raise NotImplementedError("only metric='euclidean' is supported by the B200 path yet")
+        raise NotImplementedError("only metric='euclidean' is supported by the CUDA path yet")
 
     params, reps, mod_reps, mod_n_pcs, mod_k = {}, {}, {}, {}, []
     for mod in modalities:
@@ -180,7 +180,7 @@ def neighbors(
     obs = np.asarray(mdata.obs_names).astype(str)
     for mod in modalities:
         if not np.array_equal(np.asarray(mdata.mod[mod].obs_names).astype(str), obs):
-            raise NotImplementedError("modalities with different observations are not supported by the B200 path yet")
+            raise NotImplementedError("modalities with different observations are not supported by the CUDA path yet")
     N, M = len(obs), len(modalities)
     if M > 4:
         raise NotImplementedError("more than 4 modalities")
@@ -188,9 +188,9 @@ def neighbors(
     # front instead of failing data-dependently in the middle of the call
     if M * n_multineighbors > 1536:
         raise NotImplementedError(f"n_multineighbors * modalities = {M * n_multineighbors} > 1536 candidates per cell is not "
-                                  "supported by the B200 path yet")
+                                  "supported by the CUDA path yet")
     if n_multineighbors + 1 > 320:
-        raise NotImplementedError("n_multineighbors > 319 is not supported by the B200 path yet (exact kNN kernels: k <= 320)")
+        raise NotImplementedError("n_multineighbors > 319 is not supported by the CUDA path yet (exact kNN kernels: k <= 320)")
 
     _device.require_cuda()
     dev = torch.device("cuda", torch.cuda.current_device())

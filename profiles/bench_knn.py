@@ -1,4 +1,4 @@
-"""Exact kNN, tensor-core (tcgen05 TF32 candidates + fp32 re-rank) vs SIMT kernel.  python profiles/bench_knn.py [n] [d] [k]"""
+"""Exact kNN, tensor-core (wgmma TF32 candidates + fp32 re-rank) vs SIMT kernel.  python profiles/bench_knn.py [n] [d] [k]"""
 import json
 import os
 import sys

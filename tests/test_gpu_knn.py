@@ -56,7 +56,7 @@ def test_knn_cross_and_short(cuda):
                                                   (300, 300, 7, 10, False), (1000, 2500, 128, 33, False),
                                                   (130, 100, 16, 120, True)])
 def test_tensor_core_knn_is_bit_identical_to_the_simt_kernel(cuda, nq, nc, d, k, normalise):
-    """tcgen05 TF32 candidate pass + fp32 re-rank must return exactly what the fp32 SIMT kernel returns (which is
+    """wgmma TF32 candidate pass + fp32 re-rank must return exactly what the fp32 SIMT kernel returns (which is
     itself checked against the brute-force oracle above): same indices, same distance bits, same -1 padding."""
     import torch
     from muon_b200 import _device

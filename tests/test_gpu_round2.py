@@ -279,11 +279,18 @@ def test_tiled_reduce_equals_atomic_reduce_and_counts_feed_the_transposition(cud
         assert np.array_equal(counts[c].cpu().numpy(), want), c
     # transposed panels from the reused counts == panels from the counting pass (same indptr; same entry SETS per row)
     monkeypatch.setattr(_device.TransposedPanels, "L2_BUDGET", 1 << 18)       # 1024 cells per panel at pad 64 -> 8 panels
-    monkeypatch.setenv("MUON_B200_FILL_TILED", "1")             # the atomic-free fill (opt-in: measured slower at scale)
+    monkeypatch.setenv("MUON_B200_FILL_TILED", "1")             # the deterministic tiled fill (default)
     Tp = _device.TransposedPanels(got, 64)
     Tq = _device.TransposedPanels(ref, 64)
     assert Tp.counts_reused and Tp.tiled_fill and not Tq.counts_reused and not Tq.tiled_fill
     assert len(Tp.panels) == len(Tq.panels) >= 4
+    # the tiled fill lists every transposed row in ascending cell order, identically on every build
+    Tp2 = _device.TransposedPanels(got, 64)
+    for (_, _, Ta), (_, _, Tb) in zip(Tp.panels, Tp2.panels):
+        assert torch.equal(Ta.pairs, Tb.pairs)
+        rows = torch.repeat_interleave(torch.arange(d, device=cuda), Ta.indptr[1:] - Ta.indptr[:-1])
+        key = rows * (1 << 20) + Ta.pairs[:, 0].to(torch.int64)
+        assert bool((key[1:] > key[:-1]).all())
     monkeypatch.setenv("MUON_B200_FILL_TILED", "0")
     Tr = _device.TransposedPanels(got, 64)                       # reused counts, atomic-cursor fill
     assert Tr.counts_reused and not Tr.tiled_fill

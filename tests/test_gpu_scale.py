@@ -1,6 +1,6 @@
 """GPU, BASELINE-scale shapes: size-independent properties instead of an oracle (the scipy path cannot
 hold these matrices).  400k cells x 200k peaks at 3 % = 2.4e9 non-zeros, i.e. beyond 2^31 so that every
-64-bit offset path is exercised; the full 1M-cell configuration runs in bench.py."""
+64-bit offset path is exercised.  Peak HBM: counts 19 GB + TF-IDF values 10 GB + transposed panels 19 GB."""
 import pytest
 import torch
 
@@ -16,9 +16,10 @@ N, D, DENS = 400_000, 200_000, 0.03
 
 @pytest.fixture(scope="module")
 def big(cuda):
+    torch.cuda.empty_cache()               # blocks cached by earlier tests count as used in mem_get_info
     free, _ = torch.cuda.mem_get_info()
-    if free < 120 << 30:
-        pytest.skip("needs ~120 GB of free HBM")
+    if free < 60 << 30:
+        pytest.skip("needs ~60 GB of free HBM")
     A = generate_device(N, D, DENS, tables=make_tables(D, DENS, 64, 1))
     assert A.nnz > 2**31
     return A

@@ -184,8 +184,8 @@ def test_bench_onchip_roofline_arithmetic():
     spec = importlib.util.spec_from_file_location("bench", os.path.join(os.path.dirname(__file__), "..", "bench.py"))
     bench = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(bench)
-    r = bench.onchip_roofline(nnz=6_000_000_000, P=64, ms_per_pass=88.0, sm_mhz=1920.0)
-    assert abs(r["peak"] - 148 * 128 * 1.92e9 / 1e12) < 1e-9 and r["bytes_per_nnz"] == 264.0
+    r = bench.onchip_roofline(nnz=6_000_000_000, P=64, ms_per_pass=88.0, sm_mhz=1980.0)
+    assert abs(r["peak"] - 132 * 128 * 1.98e9 / 1e12) < 1e-9 and r["bytes_per_nnz"] == 264.0
     assert abs(r["achieved"] - 6e9 * 264 / 0.088 / 1e12) < 1e-9 and 0.45 < r["frac"] < 0.55
     assert bench.onchip_roofline(1, 64, float("nan"), 1900.0) is None and bench.onchip_roofline(1, 64, 1.0, None) is None
 
