@@ -133,7 +133,8 @@ int mub_csr_transpose_fill_pairs(const int64_t* indptr, const int32_t* indices, 
  * order, so sums over it are the same on every run), for a row panel that starts on a row-block boundary: rb_count points at the
  * panel's first row block (see mub_tfidf_reduce_tiled_f32), indptr at its first row, t_indptr[n_cols+1] are the panel's
  * transposed row offsets, base is uint32 scratch [ceil(n_rows / tile height)][n_cols] (the scanned write offsets),
- * status (int32, zeroed by the caller) gets bit0 if counts and t_indptr disagree (then the result is invalid). */
+ * status (int32, zeroed by the caller) gets bit0 if counts and t_indptr disagree, or if the pattern no longer matches
+ * the counts (then the result is invalid; no slot past the panel's non-zeros is written either way). */
 int mub_csr_transpose_fill_tiled(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
                                  int32_t n_cols, const uint16_t* rb_count, const int64_t* t_indptr, uint32_t* base,
                                  int32_t* t_pairs, int32_t* status, mub_stream_t stream);

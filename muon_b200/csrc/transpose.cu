@@ -110,14 +110,39 @@ transpose_fill_pairs_kernel(const int64_t* __restrict__ indptr, const int32_t* _
 // entry count of every (512-row block, column) behind (tfidf.cu, rb_count), the write offset of block b in column c
 // is  t_indptr[c] + sum of the counts of the panel's earlier blocks  -- a column-wise scan.  Inside its block a CTA
 // sweeps the columns tile by tile; warp w owns the 32 consecutive rows [32w, 32w + 32) and walks them in order.
-// Per tile it first counts its entries per column (the columns of one row are distinct, so the lanes never collide),
-// the counts are scanned over the warps in warp order, and a second walk writes every entry at the next slot of its
-// (warp, column) cursor.  Every transposed row therefore lists its cells in ascending order, on every run.
-constexpr int kFillTileCols = 2048;    // 16 warps x 2048 columns x 4 B = 128 KB of per-warp cursors
+// Per tile it first counts its entries per column, the counts are scanned over the warps in warp order, and a second
+// walk places every entry at the next slot of its (warp, column) cursor.  Every transposed row therefore lists its
+// cells in ascending order, on every run.
+//
+// The block's slots of one column are consecutive: ~15 pairs (120 B) at 3 % density.  Written straight from the
+// walk, every lane of a warp store hits a different transposed row, so each non-zero costs an L2 write of its own,
+// and those writes, not the reads, bound the fill.  So the second walk places the tile's entries in shared memory,
+// ordered by (column, row), and the CTA then copies every (block, column) run out with consecutive lanes.  A tile
+// with more entries than the staging area holds (a dense stretch of columns) writes them straight to global memory
+// instead; the slots, hence the result, are the same.
+//
+// Loads: lane l of warp w keeps the cursor of row 32w + l in a register, and a warp issues the loads of kFillGroup
+// rows before it consumes any of them (the row starts and cursors are known, so no load waits on another).  The first
+// walk records how many entries of each row fall inside the tile, so the second walk loads exactly those.  A CTA sweeps
+// one slab of column tiles of its row block (blockIdx.y); the slab's first cursor of every row is found by a binary
+// search of the sorted row.  Slabs give every launch enough CTAs to keep two per SM busy.
+constexpr int kFillTileCols = 512;     // one column of the tile per thread in the scans
 constexpr int kFillRows = 512;         // must equal the reduce kernel's block height (mub_tfidf_tile_rows)
 constexpr int kFillThreads = 512;
 constexpr int kFillWarps = kFillThreads / 32;
 constexpr int kFillRowsPerWarp = kFillRows / kFillWarps;
+static_assert(kFillRowsPerWarp == 32, "lane l of a warp holds the cursor of the warp's row l");
+static_assert(kFillTileCols == kFillThreads, "thread j scans column j of the tile");
+constexpr int kFillGroup = 16;         // rows of a warp whose (index, value) loads are in flight together in the
+                                       // placing walk; the counting walk loads the indices of all 32 rows at once
+                                       // (~15 entries per row and tile at 3 % density: one 32-wide load each, longer
+                                       // segments continue)
+constexpr int kFillStage = 11776;      // staged pairs per tile: 1.5x the ~7.9k of a 512 x 512 tile at 3 % density
+static_assert((sizeof(int2) * kFillStage) % 16 == 0 && (sizeof(uint16_t) * kFillWarps * kFillTileCols) % 16 == 0,
+              "the cursors follow the staging area and are cleared with 16-byte stores");
+// staging + column starts + per-column write offsets + 16-bit per-warp cursors: 112 KB, two CTAs per SM
+constexpr size_t kFillSmem = sizeof(int2) * kFillStage + sizeof(uint32_t) * (2 * kFillTileCols + 1) +
+                             sizeof(uint16_t) * kFillWarps * kFillTileCols;
 
 // base[b][c] = t_indptr[c] + sum_{b' < b} count[b'][c] for the blocks of one panel (one thread per column)
 __global__ void __launch_bounds__(256)
@@ -133,72 +158,181 @@ transpose_scan_blocks_kernel(const uint16_t* __restrict__ rb_count, int32_t n_co
     if (run != (unsigned long long)t_indptr[c + 1] || run > 0xffffffffull) atomicOr(status, 1);   // counts and indptr disagree
 }
 
-__global__ void __launch_bounds__(kFillThreads, 1)
+// Besides the pairs, the kernel checks the pattern against the counts it was given: a (block, column) whose entries
+// differ from rb_count, or a row that is not sorted or holds a column >= n_cols, sets bit0 of status.  Slots at or
+// past t_indptr[n_cols] or the panel's non-zero count are never written, so a matrix modified after its counts were
+// taken cannot corrupt memory.
+__global__ void __launch_bounds__(kFillThreads, 2)
 transpose_fill_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                            const float* __restrict__ data, int64_t n_rows, int32_t n_cols,
-                            const uint32_t* __restrict__ base, int2* __restrict__ t_pairs) {
+                            const float* __restrict__ data, int64_t n_rows, int32_t n_cols, int tiles_per_slab,
+                            const uint16_t* __restrict__ rb_count, const uint32_t* __restrict__ base,
+                            const int64_t* __restrict__ t_indptr, int2* __restrict__ t_pairs, int* __restrict__ status) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    uint32_t* wcur = reinterpret_cast<uint32_t*>(smem_raw);                        // [kFillWarps][kFillTileCols]
-    int* cur = reinterpret_cast<int*>(wcur + kFillWarps * kFillTileCols);           // [kFillRows] entries done per row
-    int* ntile = cur + kFillRows;                                                   // [kFillRows] entries in this tile
+    // 16-byte aligned first: the staging area and the cursors (cleared with 16-byte stores)
+    int2* stage = reinterpret_cast<int2*>(smem_raw);                                 // [kFillStage] (column, row) order
+    uint16_t* wcur = reinterpret_cast<uint16_t*>(stage + kFillStage);                // [kFillWarps][kFillTileCols]
+    uint32_t* cstart = reinterpret_cast<uint32_t*>(wcur + kFillWarps * kFillTileCols);   // [kFillTileCols + 1] into stage
+    uint32_t* cbase = cstart + kFillTileCols + 1;                                    // [kFillTileCols] block's slot
+    __shared__ uint32_t wsum[kFillWarps];
+    constexpr unsigned kAll = 0xffffffffu;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t r0 = (int64_t)blockIdx.x * kFillRows;
-    const int rows_here = (int)((n_rows - r0) < kFillRows ? (n_rows - r0) : kFillRows);
-    const int my_r0 = warp * kFillRowsPerWarp;
-    const int my_r1 = (my_r0 + kFillRowsPerWarp < rows_here) ? my_r0 + kFillRowsPerWarp : rows_here;
-    uint32_t* my_cur = wcur + warp * kFillTileCols;
-    for (int r = threadIdx.x; r < kFillRows; r += kFillThreads) cur[r] = 0;
-    const uint32_t* my_base = base + (size_t)blockIdx.x * n_cols;
+    const int64_t row0 = r0 + warp * kFillRowsPerWarp;                              // the warp's first row
     const int n_tiles = (n_cols + kFillTileCols - 1) / kFillTileCols;
-    for (int t = 0; t < n_tiles; ++t) {
+    const int t0 = blockIdx.y * tiles_per_slab;
+    const int t1 = (t0 + tiles_per_slab < n_tiles) ? t0 + tiles_per_slab : n_tiles;
+    // slots that exist: the entries the counts announce, and no more than the panel holds (the size of t_pairs)
+    const int64_t held = __ldg(indptr + n_rows) - __ldg(indptr), announced = __ldg(t_indptr + n_cols);
+    const unsigned long long total = (unsigned long long)(announced < held ? announced : held);
+    // lane l: row row0 + l -- its first non-zero and its length
+    int64_t rs = 0;
+    int len = 0;
+    if (row0 + lane < n_rows) {
+        rs = __ldg(indptr + row0 + lane);
+        len = (int)(__ldg(indptr + row0 + lane + 1) - rs);
+    }
+    int cur = 0;
+    if (t0 > 0) {              // first entry of the slab: lower bound of its first column in the sorted row
+        const int c_first = t0 * kFillTileCols;
+        int hi = len;
+        while (cur < hi) {
+            const int mid = (int)(((unsigned)cur + (unsigned)hi) >> 1);
+            if (__ldg(indices + rs + mid) < c_first) cur = mid + 1;
+            else hi = mid;
+        }
+    }
+    int64_t rk = rs + cur;     // lane l: next entry of its row ...
+    int rem = len - cur;       // ... and the entries left in it
+    int bad = 0;
+    uint16_t* my_cur = wcur + warp * kFillTileCols;
+    uint32_t* my_cur2 = reinterpret_cast<uint32_t*>(my_cur);   // two 16-bit counters per word for the counting atomics
+    const uint32_t* blk_base = base + (size_t)blockIdx.x * n_cols;
+    const uint16_t* blk_count = rb_count + (size_t)blockIdx.x * n_cols;
+    constexpr int kCurVecs = kFillWarps * kFillTileCols * (int)sizeof(uint16_t) / 16;
+    for (int j = threadIdx.x; j < kCurVecs; j += kFillThreads) reinterpret_cast<uint4*>(wcur)[j] = make_uint4(0u, 0u, 0u, 0u);
+    __syncthreads();
+    for (int t = t0; t < t1; ++t) {
         const int c_lo = t * kFillTileCols;
         const int c_hi = (c_lo + kFillTileCols < n_cols) ? c_lo + kFillTileCols : n_cols;
-        for (int j = threadIdx.x; j < kFillWarps * kFillTileCols; j += kFillThreads) wcur[j] = 0;
-        __syncthreads();
-        // walk 1: entries per (warp, column) of this tile, and per row the number of its entries inside the tile
-        for (int r = my_r0; r < my_r1; ++r) {
-            const int64_t e = __ldg(indptr + r0 + r + 1);
-            const int64_t k0 = __ldg(indptr + r0 + r) + cur[r];
-            int64_t k = k0;
-            for (;;) {
-                const int c = k + lane < e ? ld_stream(indices + k + lane) : 0x7fffffff;
-                const bool in = c < c_hi;                  // sorted row: the entries of this tile come first
-                const int n_in = __popc(__ballot_sync(0xffffffffu, in));
-                if (in && c >= c_lo) my_cur[c - c_lo] += 1;
-                k += n_in;
+        // thread j's operands of the scan below (column c_lo + j), in flight during the first walk
+        const bool col_in = c_lo + (int)threadIdx.x < c_hi;
+        const uint32_t want = col_in ? (uint32_t)__ldg(blk_count + c_lo + threadIdx.x) : 0u;
+        const uint32_t slot0 = col_in ? __ldg(blk_base + c_lo + threadIdx.x) : 0u;
+        // walk 1: entries per (warp, column) of this tile, and per row (lane) the number of its entries inside the tile
+        int ntile = 0;
+        int c[kFillRowsPerWarp];
+#pragma unroll
+        for (int i = 0; i < kFillRowsPerWarp; ++i) {
+            const int64_t s = __shfl_sync(kAll, rk, i);
+            const int n = __shfl_sync(kAll, rem, i);
+            c[i] = lane < n ? __ldg(indices + s + lane) : 0x7fffffff;
+        }
+#pragma unroll
+        for (int i = 0; i < kFillRowsPerWarp; ++i) {
+            int cc = c[i], taken = 0;
+            for (int k = 0;;) {
+                const bool in = cc < c_hi;
+                const unsigned m = __ballot_sync(kAll, in);
+                const int n_in = __popc(m);
+                // sorted row: the tile's entries are a prefix of what follows the cursor, all >= c_lo
+                bad |= (m != (n_in == 32 ? kAll : (1u << n_in) - 1u)) | (in && cc < c_lo);
+                if (in && cc >= c_lo) atomicAdd(my_cur2 + ((cc - c_lo) >> 1), 1u << (16 * ((cc - c_lo) & 1)));
+                taken += n_in;
                 if (n_in < 32) break;
+                // the row's segment is longer than the load issued up front
+                k += 32;
+                const int64_t s = __shfl_sync(kAll, rk, i);
+                const int n = __shfl_sync(kAll, rem, i);
+                cc = k + lane < n ? __ldg(indices + s + k + lane) : 0x7fffffff;
             }
-            if (lane == 0) ntile[r] = (int)(k - k0);
+            if (lane == i) ntile = taken;
         }
         __syncthreads();
-        // exclusive scan over the warps, in warp (= row) order, from the block's write offset of each column
-        for (int j = threadIdx.x; j < c_hi - c_lo; j += kFillThreads) {
-            uint32_t run = my_base[c_lo + j];
+        // thread j, column c_lo + j: exclusive scan over the warps, in warp (= row) order; the block's total must be
+        // the count the write offsets were scanned from.  Then an exclusive scan of the totals over the tile's
+        // columns places every column's run in the staging area.
+        {
+            const int j = threadIdx.x;
+            uint32_t run = 0;
 #pragma unroll
             for (int w = 0; w < kFillWarps; ++w) {
                 const uint32_t cnt = wcur[w * kFillTileCols + j];
-                wcur[w * kFillTileCols + j] = run;
+                wcur[w * kFillTileCols + j] = (uint16_t)run;
                 run += cnt;
             }
+            if (col_in) {
+                bad |= run != want;
+                cbase[j] = slot0;
+            }
+            uint32_t x = run;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t y = __shfl_up_sync(kAll, x, d);
+                if (lane >= d) x += y;
+            }
+            if (lane == 31) wsum[warp] = x;
+            __syncthreads();
+            uint32_t off = 0;
+            for (int w = 0; w < warp; ++w) off += wsum[w];
+            cstart[j] = off + x - run;
+            if (j == kFillTileCols - 1) cstart[kFillTileCols] = off + x;
         }
         __syncthreads();
-        // walk 2: rows in order, each entry at the next slot of its (warp, column) cursor
-        for (int r = my_r0; r < my_r1; ++r) {
-            const int64_t k0 = __ldg(indptr + r0 + r) + cur[r];
-            const int n = ntile[r];
-            for (int i = lane; i < n; i += 32) {
-                const int c = ld_stream(indices + k0 + i);
-                const float v = ld_stream(data + k0 + i);
-                if (c >= c_lo) {
-                    const uint32_t slot = my_cur[c - c_lo]++;
-                    t_pairs[slot] = make_int2((int)(r0 + r), __float_as_int(v));
-                }
+        const bool staged = cstart[kFillTileCols] <= (uint32_t)kFillStage;          // CTA-uniform
+        // walk 2: rows in order, each entry at the next slot of its (warp, column) cursor; the loads of a group of
+        // rows are issued before the first of them is placed
+        auto place = [&](int j, int r, float v) {
+            const uint32_t o = my_cur[j]++;                // slot within the block's run of column c_lo + j
+            if (staged) {
+                const uint32_t p = cstart[j] + o;
+                if (p < cstart[j + 1]) stage[p] = make_int2(r, __float_as_int(v));
+            } else {
+                const uint32_t slot = cbase[j] + o;
+                if (slot < total) t_pairs[slot] = make_int2(r, __float_as_int(v));
             }
-            __syncwarp();
-            if (lane == 0) cur[r] += n;
+        };
+        for (int g = 0; g < kFillRowsPerWarp; g += kFillGroup) {
+            int c[kFillGroup];
+            float v[kFillGroup];
+#pragma unroll
+            for (int i = 0; i < kFillGroup; ++i) {
+                const int64_t s = __shfl_sync(kAll, rk, g + i);
+                const int n = __shfl_sync(kAll, ntile, g + i);
+                c[i] = lane < n ? ld_stream(indices + s + lane) : -1;
+                v[i] = lane < n ? ld_stream(data + s + lane) : 0.f;
+            }
+#pragma unroll
+            for (int i = 0; i < kFillGroup; ++i) {
+                const int r = (int)(row0 + g + i);         // panel-local row index, as indptr starts at the panel
+                if (c[i] >= c_lo && c[i] < c_hi) place(c[i] - c_lo, r, v[i]);
+                const int n = __shfl_sync(kAll, ntile, g + i);
+                if (n > 32) {
+                    const int64_t s = __shfl_sync(kAll, rk, g + i);
+                    for (int k = 32 + lane; k - lane < n; k += 32) {
+                        const int cc = k < n ? ld_stream(indices + s + k) : -1;
+                        const float vv = k < n ? ld_stream(data + s + k) : 0.f;
+                        if (cc >= c_lo && cc < c_hi) place(cc - c_lo, r, vv);
+                    }
+                }
+                __syncwarp();                              // row r's cursor updates land before row r + 1 reads them
+            }
         }
+        rk += ntile;
+        rem -= ntile;
+        __syncthreads();
+        // every (block, column) run out of the staging area by consecutive lanes; cursors back to zero for the next tile
+        if (staged) {
+            for (int j = warp; j < c_hi - c_lo; j += kFillWarps) {
+                const uint32_t p0 = cstart[j], n = cstart[j + 1] - p0, g0 = cbase[j];
+                for (uint32_t e = lane; e < n; e += 32)
+                    if (g0 + e < total) t_pairs[g0 + e] = stage[p0 + e];
+            }
+        }
+        for (int j = threadIdx.x; j < kCurVecs; j += kFillThreads) reinterpret_cast<uint4*>(wcur)[j] = make_uint4(0u, 0u, 0u, 0u);
         __syncthreads();
     }
+    if (t1 == n_tiles) bad |= rem != 0;                  // entries left over: a column >= n_cols (or unsorted)
+    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(status, 1);
 }
 
 __global__ void __launch_bounds__(256)
@@ -342,13 +476,22 @@ extern "C" int mub_csr_transpose_fill_tiled(const int64_t* indptr, const int32_t
     const int64_t n_blocks = (n_rows + mub::kFillRows - 1) / mub::kFillRows;
     MUB_REQUIRE(n_blocks < (1ll << 31), "transpose_fill_tiled: too many rows");
     mub::transpose_scan_blocks_kernel<<<(n_cols + 255) / 256, 256, 0, s>>>(rb_count, n_cols, n_blocks, t_indptr, base, status);
-    const size_t smem = sizeof(uint32_t) * mub::kFillWarps * mub::kFillTileCols + 2 * sizeof(int) * mub::kFillRows;
+    const size_t smem = mub::kFillSmem;
     cudaError_t e = cudaFuncSetAttribute(mub::transpose_fill_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess)      // room for two CTAs per SM
+        e = cudaFuncSetAttribute(mub::transpose_fill_tiled_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 (int)cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) {
         mub::set_error("transpose_fill_tiled: %zu B of shared memory: %s", smem, cudaGetErrorString(e));
         return -2;
     }
-    mub::transpose_fill_tiled_kernel<<<(int)n_blocks, mub::kFillThreads, smem, s>>>(indptr, indices, data, n_rows, n_cols, base,
-                                                                                  (int2*)t_pairs);
+    // column slabs per row block: about 8 CTAs per SM in all, so that the last wave is short
+    const int n_tiles = (int)((n_cols + mub::kFillTileCols - 1) / mub::kFillTileCols);
+    int64_t slabs = (8ll * mub::sm_count() + n_blocks - 1) / n_blocks;
+    slabs = slabs < 1 ? 1 : (slabs > n_tiles ? n_tiles : slabs);
+    const int tiles_per_slab = (int)((n_tiles + slabs - 1) / slabs);
+    const dim3 grid((unsigned)n_blocks, (unsigned)((n_tiles + tiles_per_slab - 1) / tiles_per_slab));
+    mub::transpose_fill_tiled_kernel<<<grid, mub::kFillThreads, smem, s>>>(indptr, indices, data, n_rows, n_cols, tiles_per_slab,
+                                                                          rb_count, base, t_indptr, (int2*)t_pairs, status);
     return mub::check_launch("transpose_fill_tiled");
 }
