@@ -197,6 +197,33 @@ int mub_mofa_pseudo_f32(float* zeta, const float* obs, const float* kappa, int64
 int mub_mofa_loglik_f32(const float* zeta, const float* obs, int64_t n_rows, int32_t D, int32_t kind, double* out,
                         mub_stream_t stream);
 
+/* The same quantities for a SPARSE view, without materialising anything N x D.  With g(zeta) = zeta - sigmoid(zeta)
+ * / kappa_d the pseudo-data are yhat = g(zeta) everywhere plus, at the stored entries only, s = y sigmoid(zeta) /
+ * (kappa_d r(zeta)) (poisson, r = max(ln(1+e^zeta), 1e-30)) or s = y / kappa_d (bernoulli); ln p is -r(zeta)
+ * (poisson) / -ln(1+e^zeta) (bernoulli) everywhere plus y ln r(zeta) / y zeta at the stored entries.
+ * zeta = Z W^T for Z[n x ld], W[D x ld] (padded columns zero), ld in {32, 64}.  fp32 arithmetic as mub_mofa_pseudo_f32;
+ * sums of ln p and of squares in fp64.  A call with n = 0 or D = 0 writes nothing.
+ *   lowrank_rows : B[D x ld] given: out[n x ld] = g(zeta) B (accumulate = 0) or += (1), each output row written once,
+ *                  deterministic.  B = NULL: *loglik += the everywhere-part of sum ln p (kappa, out unused).
+ *   lowrank_cols : P[D x ld] = g(zeta)^T C for C[n x ld] (C = Z gives Yhat^T Z), ssq[D] = sum_n g(zeta)^2; both
+ *                  written, deterministic.
+ *   nnz_rows     : CSR of the observations (n_rows = n cells); B given: out[n x ld] += S B; B = NULL: *loglik += the
+ *                  stored-entry part of sum ln p.
+ *   nnz_cols     : one transposed row panel of the observations in the pairs layout (mub_csr_transpose_fill_pairs):
+ *                  D rows, entries indexed by the panel's cells, Z and C pointing at the panel's first cell;
+ *                  P[D x ld] += S^T C and ssq[D] += sum (2 g s + s^2) over the entries (the cross terms of sum yhat^2). */
+int mub_mofa_lowrank_rows_f32(const float* Z, int64_t n, const float* W, int64_t D, const float* kappa, const float* B,
+                              int32_t ld, int32_t kind, float* out, int32_t accumulate, double* loglik,
+                              mub_stream_t stream);
+int mub_mofa_lowrank_cols_f32(const float* Z, int64_t n, const float* W, int64_t D, const float* kappa, const float* C,
+                              int32_t ld, int32_t kind, float* P, double* ssq, mub_stream_t stream);
+int mub_mofa_nnz_rows_f32(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
+                          const float* Z, const float* W, const float* kappa, const float* B, int32_t ld, int32_t kind,
+                          float* out, double* loglik, mub_stream_t stream);
+int mub_mofa_nnz_cols_f32(const int64_t* t_indptr, const int32_t* t_pairs, int64_t D, const float* Z, const float* W,
+                          const float* kappa, const float* C, int32_t ld, int32_t kind, float* P, double* ssq,
+                          mub_stream_t stream);
+
 
 /* ---- exact k-nearest neighbours (groundwork for the WNN row, muon/_core/preproc.py:520-528: the reference asks
  * umap's NN-descent for n_multineighbors+1 = 201 neighbours per cell and modality; this search is exact).

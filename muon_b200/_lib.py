@@ -47,6 +47,10 @@ SIGNATURES = {
     "mub_mofa_tau_f32": [vp, vp, vp, f64, vp, vp, vp, vp, f64, vp, i64, i32, i32, vp],
     "mub_mofa_pseudo_f32": [vp, vp, vp, i64, i32, i32, vp],
     "mub_mofa_loglik_f32": [vp, vp, i64, i32, i32, vp, vp],
+    "mub_mofa_lowrank_rows_f32": [vp, i64, vp, i64, vp, vp, i32, i32, vp, i32, vp, vp],
+    "mub_mofa_lowrank_cols_f32": [vp, i64, vp, i64, vp, vp, i32, i32, vp, vp, vp],
+    "mub_mofa_nnz_rows_f32": [vp, vp, vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp],
+    "mub_mofa_nnz_cols_f32": [vp, vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp],
     "mub_knn_l2_f32": [vp, i64, vp, i64, i32, i32, i32, vp, vp, vp],
     "mub_knn_l2_tc_f32": [vp, i64, vp, i64, i32, i32, i32, vp, vp, vp, C.c_size_t, vp, vp],
     "mub_wnn_bandwidth_f32": [vp, vp, vp, vp, vp, i64, i32, i32, i32, f64, vp, vp, vp, i64, vp, i32, i32, vp],

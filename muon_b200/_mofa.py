@@ -11,8 +11,11 @@ sharded across ranks; ``P``, the K x K Gram and K-vectors are sum-allreduced (SU
 The update equations and their order are those of oracle/mofa_ref.py (see its header for the
 parity status against mofapy2).
 
-Supported: gaussian views kept sparse (implicit centring), poisson / bernoulli views as dense Seeger pseudo-data
-(guessed from the data like mofapy2 does when ``likelihoods=None``), ``groups_label``, ``use_obs`` union /
+Supported: gaussian views kept sparse (implicit centring), poisson / bernoulli views (guessed from the data like mofapy2
+does when ``likelihoods=None``) through Seeger pseudo-data -- dense when they fit in 60 % of the free device memory,
+else, for a sparse input, never stored: g(zeta) over all cells x features plus a correction at the stored entries,
+evaluated by fused low-rank kernels (csrc/mofa_lowrank.cu; ``MUON_B200_MOFA_PSEUDO`` = auto / dense / sparse, the
+path taken is recorded in ``uns["mofa"]["_b200"]["pseudo"]``), ``groups_label``, ``use_obs`` union /
 intersection (cells missing from whole views), ``use_var`` feature subsets, ``use_layer``, ``scale_views``,
 ``scale_groups``, ``center_groups``, ARD on weights / factors, spike-and-slab weights, convergence modes, ``copy``;
 the one-group case also cell-sharded over several GPUs.  Not supported (``NotImplementedError``, never a silent
@@ -21,6 +24,7 @@ available); ``n_factors`` > 64.
 """
 from __future__ import annotations
 
+import os
 from functools import reduce
 from typing import Optional
 from warnings import warn
@@ -98,6 +102,85 @@ class _DenseBlock:
             Q.index_add_(0, self.rows, self.Y @ tw)
 
 
+def _padded(X, K):
+    """contiguous copy of X[:, :K] with the padded columns zero (the layout the low-rank kernels read)"""
+    out = torch.zeros_like(X)
+    out[:, :K] = X[:, :K]
+    return out
+
+
+class _SparsePseudoBlock:
+    """One (view, group) block of a NON-gaussian view kept sparse: the observations as a CSR with its transpose panels.
+    The pseudo-data are never stored.  They are g(zeta) everywhere plus a correction s at the stored entries
+    (csrc/mofa_lowrank.cu), with zeta = Z_zeta W_zeta^T at the factors the current pseudo-data were formed at, so a
+    copy of those factors is kept.  Contractions: a low-rank sweep for the g part plus a gathering pass over the
+    non-zeros."""
+
+    def __init__(self, A: _device.DeviceCSR, rows, lo: int, hi: int, ld: int, kind: int):
+        self.A, self.At = A, A.transpose_panels(ld)
+        self.rows, self.lo, self.hi = rows, lo, hi
+        self.n_local = A.shape[0]
+        self.ld, self.kind = ld, kind
+        self.Zz = self.Wz = self.kappa = None            # no pseudo-data formed yet: Yhat = 0
+
+    def take(self, Z):
+        return Z[self.lo:self.hi] if self.rows is None else Z.index_select(0, self.rows)
+
+    def col_max(self, D, dev):
+        """max over the block's cells of every feature, implicit zeros counting as 0"""
+        mx = torch.zeros(D, dtype=torch.float32, device=dev)
+        step = 1 << 26                                      # bounds the int64 copy of the indices
+        for k0 in range(0, self.A.nnz, step):
+            k1 = min(self.A.nnz, k0 + step)
+            mx.scatter_reduce_(0, self.A.indices[k0:k1].to(torch.int64), self.A.data[k0:k1], "amax")
+        return mx
+
+    def pseudo(self, Zb, W, kappa, K):
+        """form the pseudo-data at zeta = Zb W^T; return (Yhat^T Zb, sum_n Yhat^2 per feature)"""
+        self.Zz, self.Wz, self.kappa = _padded(Zb, K), _padded(W, K), kappa
+        return self._aty(self.Zz)
+
+    def aty(self, Zb):
+        if self.Zz is None:
+            return torch.zeros((self.At.shape[0], self.ld), dtype=torch.float32, device=Zb.device)
+        return self._aty(Zb.contiguous())[0]
+
+    def _aty(self, C):
+        """(Yhat^T C, sum_n Yhat^2 per feature)"""
+        D, n, st = self.At.shape[0], self.n_local, stream_ptr()
+        P = torch.empty((D, self.ld), dtype=torch.float32, device=C.device)
+        ssq = torch.empty(D, dtype=f64, device=C.device)
+        call("mub_mofa_lowrank_cols_f32", ptr(self.Zz), n, ptr(self.Wz), D, ptr(self.kappa), ptr(C), self.ld, self.kind,
+             ptr(P), ptr(ssq), st)
+        self.At.wait()
+        row = 4 * self.ld
+        for r0, _, T in self.At.panels:
+            call("mub_mofa_nnz_cols_f32", ptr(T.indptr), ptr(T.pairs), D, ptr(self.Zz) + row * r0, ptr(self.Wz),
+                 ptr(self.kappa), ptr(C) + row * r0, self.ld, self.kind, ptr(P), ptr(ssq), st)
+        return P, ssq
+
+    def add_av(self, Q, tw):                             # Q[rows of the block] += Yhat (tau * W)
+        n, D, st = self.n_local, self.At.shape[0], stream_ptr()
+        out = Q[self.lo:self.hi] if self.rows is None else torch.zeros((n, self.ld), dtype=torch.float32, device=Q.device)
+        call("mub_mofa_lowrank_rows_f32", ptr(self.Zz), n, ptr(self.Wz), D, ptr(self.kappa), ptr(tw), self.ld, self.kind,
+             ptr(out), 1, None, st)
+        if self.kind == 2:                               # bernoulli: s = y / kappa is linear in y
+            _device.spmm(self.A, (tw / self.kappa[:, None]).contiguous(), out=out, accumulate=True, dynamic=False)
+        else:
+            call("mub_mofa_nnz_rows_f32", ptr(self.A.indptr), ptr(self.A.indices), ptr(self.A.data), n, ptr(self.Zz),
+                 ptr(self.Wz), ptr(self.kappa), ptr(tw), self.ld, self.kind, ptr(out), None, st)
+        if self.rows is not None:
+            Q.index_add_(0, self.rows, out)
+
+    def loglik(self, Zb, W, K, acc):
+        """acc += sum over the block's cells and all features of ln p(y | zeta) at zeta = Zb W^T"""
+        Zp, Wp, st = _padded(Zb, K), _padded(W, K), stream_ptr()
+        call("mub_mofa_lowrank_rows_f32", ptr(Zp), self.n_local, ptr(Wp), Wp.shape[0], None, None, self.ld, self.kind,
+             None, 0, ptr(acc), st)
+        call("mub_mofa_nnz_rows_f32", ptr(self.A.indptr), ptr(self.A.indices), ptr(self.A.data), self.n_local, ptr(Zp),
+             ptr(Wp), None, None, self.ld, self.kind, None, ptr(acc), st)
+
+
 class _View:
     """One modality: blocks per group, per-(group, feature) moments, variational state of W / alpha / theta / tau."""
 
@@ -117,6 +200,8 @@ class _View:
                 continue
             if self.kind == 0:
                 s1[g], s2[g] = b.moments(D, dev)
+            elif isinstance(b, _SparsePseudoBlock):
+                mx = torch.maximum(mx, b.col_max(D, dev))
             else:
                 mx = torch.maximum(mx, b.obs.max(0).values)
         if self.kind != 0:
@@ -250,6 +335,8 @@ class MofaDevice:
                 r, lo, hi = (None, rows[0], rows[1]) if isinstance(rows, tuple) else (rows, 0, 0)
                 if self.liks[m] == "gaussian":
                     bl.append(_Block(A, r, lo, hi, ld))
+                elif isinstance(A, _device.DeviceCSR):    # non-gaussian view kept sparse
+                    bl.append(_SparsePseudoBlock(A, r, lo, hi, ld, 1 if self.liks[m] == "poisson" else 2))
                 else:                                     # A: dense fp32 observations (n_b x D) on the device
                     bl.append(_DenseBlock(A, r, lo, hi))
             self.views.append(_View(bl, dims[m], K, ld, center, scale_views, scale_groups, dev, self.liks[m]))
@@ -269,20 +356,25 @@ class MofaDevice:
         K = self.K
         dK = torch.arange(K, device=self.dev)
         for m, v in enumerate(self.views):
+            # Yhat^T E[Z] of a sparse non-gaussian view is read only by variance_explained() (the next _pseudo
+            # overwrites it), so it is formed there, once, instead of a low-rank sweep per iteration
+            v.P_stale = any(isinstance(b, _SparsePseudoBlock) for b in v.blocks)
             for g, b in enumerate(v.blocks):
                 if b.n_local > 0:
                     Zb = b.take(self.Z)
                     ZZ = _device.gram(Zb, K, reduce=False)
                     zs = Zb[:, :K].sum(0, dtype=f64)
-                    P = b.aty(Zb.contiguous())
+                    if not v.P_stale:
+                        v.P[g] = b.aty(Zb.contiguous())
                 else:
                     ZZ = torch.zeros((K, K), dtype=f64, device=self.dev)
                     zs = torch.zeros(K, dtype=f64, device=self.dev)
-                    P = torch.zeros((v.D, self.ld), dtype=torch.float32, device=self.dev)
-                v.ZZ_mean[g], v.zsum[g], v.P[g] = ZZ, zs, P
+                    v.P[g] = 0.0
+                v.ZZ_mean[g], v.zsum[g] = ZZ, zs
             _dist.all_reduce_sum_(v.ZZ_mean)
             _dist.all_reduce_sum_(v.zsum)
-            _dist.all_reduce_sum_(v.P)
+            if not v.P_stale:
+                _dist.all_reduce_sum_(v.P)
             v.ZZ = v.ZZ_mean.clone()
             for g in range(self.G):
                 cl = self._class_members(m, g)
@@ -371,6 +463,9 @@ class MofaDevice:
                 v.ssq[g].zero_()
                 continue
             Zb = b.take(self.Z).contiguous()
+            if isinstance(b, _SparsePseudoBlock):
+                v.P[g], v.ssq[g] = b.pseudo(Zb, v.W, v.kappa32, K)
+                continue
             torch.matmul(Zb[:, :K], Wk.T, out=b.Y)
             call("mub_mofa_pseudo_f32", ptr(b.Y), ptr(b.obs), ptr(v.kappa32), b.n_local, v.D, v.kind, st)
             v.P[g] = b.aty(Zb)
@@ -385,6 +480,9 @@ class MofaDevice:
         Wk = v.W[:, :K].contiguous()
         for b in v.blocks:
             if b.n_local == 0:
+                continue
+            if isinstance(b, _SparsePseudoBlock):
+                b.loglik(b.take(self.Z), v.W, K, acc)
                 continue
             zeta = b.take(self.Z)[:, :K].contiguous() @ Wk.T
             call("mub_mofa_loglik_f32", ptr(zeta), ptr(b.obs), b.n_local, v.D, v.kind, ptr(acc), st)
@@ -439,6 +537,12 @@ class MofaDevice:
         K = self.K
         out = []
         for v in self.views:
+            if v.P_stale:
+                for g, b in enumerate(v.blocks):
+                    if b.n_local > 0:
+                        v.P[g] = b.aty(b.take(self.Z))
+                _dist.all_reduce_sum_(v.P)
+                v.P_stale = False
             W = v.W[:, :K].to(f64)
             r2 = torch.zeros((self.G, K), dtype=f64, device=self.dev)
             for g in range(self.G):
@@ -519,6 +623,20 @@ def _guess_likelihood(X) -> str:
     return "bernoulli" if np.all((vals == 0) | (vals == 1)) else "poisson"
 
 
+def _pseudo_path(sparse_input: bool, shape, free_bytes: int, mode: str) -> str:
+    """How a poisson / bernoulli view is held: "dense" (observations, pseudo-data and zeta as dense fp32 matrices, 12 B
+    per element) or "sparse" (the observations' CSR; the pseudo-data never stored).  ``mode`` is
+    $MUON_B200_MOFA_PSEUDO: "dense" and "sparse" force a path (a dense input is converted to CSR on the host for
+    "sparse"); "auto" keeps the dense path whenever it fits in 60 % of the free device memory, else takes the sparse
+    one if the input is sparse (a dense input that does not fit keeps the dense path, which refuses it)."""
+    if mode not in ("auto", "dense", "sparse"):
+        raise ValueError(f"MUON_B200_MOFA_PSEUDO must be 'auto', 'dense' or 'sparse', got {mode!r}")
+    if mode != "auto":
+        return mode
+    fits = 12.0 * shape[0] * shape[1] <= 0.6 * free_bytes
+    return "dense" if fits or not sparse_input else "sparse"
+
+
 def _check_dense_fits(name, shape, lik, dev):
     """Non-gaussian views need dense N x D pseudo-data (observations + pseudo-data + zeta: 12 B per element)."""
     need = 12.0 * shape[0] * shape[1]
@@ -528,6 +646,20 @@ def _check_dense_fits(name, shape, lik, dev):
             f"view '{name}' ({shape[0]} x {shape[1]}) was given / guessed the {lik} likelihood, whose pseudo-data are dense by "
             f"construction: {need / 2**30:.0f} GiB needed, {free / 2**30:.0f} GiB free on the device (the reference densifies "
             "every view and cannot run this size either).  Pass likelihoods='gaussian' for normalised data, or subset.")
+
+
+def _to_sparse_pseudo_view(X) -> _device.DeviceCSR:
+    """Observations of a non-gaussian view kept sparse: a DeviceCSR stays where it is, anything else is uploaded as CSR
+    (a dense host array converted on the host first)."""
+    import scipy.sparse as sp
+    if isinstance(X, torch.Tensor):
+        X = X.cpu().numpy()
+    vals = X.data if isinstance(X, _device.DeviceCSR) or sp.issparse(X) else np.asarray(X)
+    nan = bool(torch.isnan(vals).any()) if isinstance(vals, torch.Tensor) else bool(np.isnan(vals).any())
+    if nan:
+        raise NotImplementedError("missing values (NaN) inside a non-gaussian view are not supported; drop the cells "
+                                  "from the view and use use_obs='union'")
+    return _to_device_view(X)
 
 
 def _to_dense_device(X, dev) -> torch.Tensor:
@@ -660,12 +792,20 @@ def mofa(
         # The reference lets mofapy2 guess the likelihood per view (tools.py:272-280, mofapy2 guess_likelihoods):
         # all values in {0,1} -> bernoulli, all integers -> poisson, else gaussian.
         lik = [_guess_likelihood(X) for X in Xs]
+    mode = os.environ.get("MUON_B200_MOFA_PSEUDO", "auto")
+    free = torch.cuda.mem_get_info(dev)[0]
+    pseudo = {}
     for m, X, l in zip(mods, Xs, lik):
         if l != "gaussian":
-            _check_dense_fits(m, X.shape, l, dev)
+            pseudo[m] = _pseudo_path(isinstance(X, _device.DeviceCSR) or sp.issparse(X), X.shape, free, mode)
+            if pseudo[m] == "dense":
+                _check_dense_fits(m, X.shape, l, dev)
+
+    def pseudo_obs(m, X):                                 # observations of a poisson / bernoulli view (or block)
+        return _to_dense_device(X, dev) if pseudo[m] == "dense" else _to_sparse_pseudo_view(X)
 
     if simple:
-        views = [_to_device_view(X) if l == "gaussian" else _to_dense_device(X, dev) for X, l in zip(Xs, lik)]
+        views = [_to_device_view(X) if l == "gaussian" else pseudo_obs(m, X) for m, X, l in zip(mods, Xs, lik)]
         sparse_views = [v for v in views if isinstance(v, _device.DeviceCSR)]
         n_local = views[0].shape[0]
         if sparse_views:
@@ -723,7 +863,7 @@ def mofa(
                 if lik[mi] == "gaussian":
                     A = _device.DeviceCSR.from_scipy(sp.csr_matrix(Xg), dtype=np.float32)
                 else:
-                    A = _to_dense_device(Xg, dev)
+                    A = pseudo_obs(m, Xg)
                 if len(rows_z) == hi - lo and np.array_equal(rows_z, np.arange(lo, hi)):
                     per_g.append((A, (lo, hi)))
                 else:
@@ -770,7 +910,8 @@ def mofa(
         },
         "variance": variance,
     }
-    data.uns["mofa"]["_b200"] = {"iterations": res["iterations"], "converged": res["converged"], "elbo": res["elbo"]}
+    data.uns["mofa"]["_b200"] = {"iterations": res["iterations"], "converged": res["converged"], "elbo": res["elbo"],
+                                 "pseudo": pseudo}
     if copy:
         return data
     if not quiet:
