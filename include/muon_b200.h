@@ -99,14 +99,6 @@ int mub_spmm_csr_f32(const int64_t* indptr, const int32_t* indices, const float*
                      int64_t n_rows, int64_t n_cols, const float* B, int32_t ld, float* C,
                      int32_t accumulate, unsigned long long* row_counter, mub_stream_t stream);
 
-/* Same product, shared-memory staged variant for matrices whose column indices are SORTED within
- * each row (canonical CSR): column panels of B are TMA-copied (cp.async.bulk) into shared memory
- * behind mbarriers and a persistent CTA sweeps a block of rows over them with register-resident
- * accumulators, cutting the L2->SM gather traffic of the row-warp kernel.  Deterministic. */
-int mub_spmm_csr_panel_f32(const int64_t* indptr, const int32_t* indices, const float* data,
-                           int64_t n_rows, int64_t n_cols, const float* B, int32_t ld, float* C,
-                           int32_t accumulate, mub_stream_t stream);
-
 /* ---- CSR transpose (one-time per matrix): builds the CSR of A^T so that A^T * Y is again a
  * row-gather SpMM (scipy does the same implicitly through csc_matvec, _svds.py:447).
  * Step 1 counts entries per column into t_count[n_cols+1] (int64, zeroed by caller, slot 0 unused
@@ -125,7 +117,8 @@ int mub_csr_transpose_fill(const int64_t* indptr, const int32_t* indices, const 
  * so the scatter writes once per non-zero and the product reads one 8-byte word per entry.
  * fill_pairs: like mub_csr_transpose_fill, writing t_pairs[2*nnz] (int32 view of the int2 array).
  * spmm_csrp : C (+)= A B for a pairs-layout matrix (same kernel family and rules as mub_spmm_csr_f32).
- * csrp_row_stats: mub_csr_row_stats_f32 on the pairs layout. */
+ * csrp_row_stats: per-row sum and sum of squares (fp64).  On the transposed panels these are the per-feature
+ *                 moments behind MOFA's centring / intercepts (muon/_core/tools.py:283-287, mofapy2 process_data). */
 int mub_csr_transpose_fill_pairs(const int64_t* indptr, const int32_t* indices, const float* data,
                                  int64_t n_rows, int32_t n_cols, int64_t row_offset, const int64_t* t_indptr,
                                  int64_t* cursor, int32_t* t_pairs, mub_stream_t stream);
@@ -143,11 +136,6 @@ int mub_spmm_csrp_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_row
                       mub_stream_t stream);
 int mub_csrp_row_stats_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, double* sum,
                            double* sumsq, mub_stream_t stream);
-
-/* per-row sum and sum of squares of a CSR (fp64).  On the CSR of A^T these are the per-feature
- * moments behind MOFA's centring / intercepts (muon/_core/tools.py:283-287, mofapy2 process_data). */
-int mub_csr_row_stats_f32(const int64_t* indptr, const float* data, int64_t n_rows, double* sum,
-                          double* sumsq, mub_stream_t stream);
 
 /* ---- tall-skinny Gram (the k x k contraction that is allreduced across cell shards) ------
  * G[l x l] = Y^T Y for Y[n x ld] row-major, float64 result (partials are fp32 per CTA slab,

@@ -360,10 +360,10 @@ class DeviceCSR:
             self._t = csr_transpose(self)
         return self._t
 
-    def transpose_panels(self, pad: int = 64, side_stream: bool = False) -> "TransposedPanels":
+    def transpose_panels(self, pad: int = 64) -> "TransposedPanels":
         key = ("panels", pad)
         if getattr(self, "_tp", None) is None or self._tp[0] != key:
-            self._tp = (key, TransposedPanels(self, pad, side_stream))
+            self._tp = (key, TransposedPanels(self, pad))
         return self._tp[1]
 
 
@@ -531,7 +531,7 @@ class TransposedPanels:
     # bytes of the gathered operand per panel (H100 L2: 50 MB, shared with the CSR stream)
     L2_BUDGET = int(os.environ.get("MUON_B200_L2_BUDGET_MB", "16")) << 20
 
-    def __init__(self, A: DeviceCSR, pad: int = 64, side_stream: bool = False):
+    def __init__(self, A: DeviceCSR, pad: int = 64):
         n = A.shape[0]
         rows = max(1, self.L2_BUDGET // (4 * pad))
         n_panels = max(1, -(-n // rows))
@@ -550,7 +550,7 @@ class TransposedPanels:
                 # the tiled fill lists every transposed row in ascending cell order, so A^T Y sums in the same
                 # order on every run (the atomic-cursor fill's order follows slot claims); MUON_B200_FILL_TILED=0
                 # selects the atomic-cursor fill
-                if os.environ.get("MUON_B200_FILL_TILED", "1") == "1" and not side_stream:
+                if os.environ.get("MUON_B200_FILL_TILED", "1") == "1":
                     rb = aux.get("rb_counts")
         else:
             bounds = [round(i * n / n_panels) for i in range(n_panels + 1)]
@@ -559,66 +559,31 @@ class TransposedPanels:
         self.shape = (A.shape[1], n)
         # non-zero offsets of the panel boundaries: one small D2H up front, no host syncs afterwards
         ks = A.indptr[torch.tensor(bounds, device=A.indptr.device)].tolist()
-        self.ready = None
-        if side_stream:
-            # build on a second stream so that the first A*V product (main stream) overlaps it;
-            # consumers call wait() before touching the panels
-            main = torch.cuda.current_stream()
-            side = torch.cuda.Stream()
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                self.panels = [(bounds[i], bounds[i + 1], csr_transpose(A, bounds[i], bounds[i + 1], ks[i], ks[i + 1], pairs=True,
-                                                                        col_count=counts[i] if counts else None))
-                               for i in range(n_panels)]
-                self.ready = side.record_event()
-            for _, _, T in self.panels:           # memory is consumed on the main stream later on
-                for t in (T.indptr, T.pairs):
-                    t.record_stream(main)
-        else:
-            scratch = {}
-            build = lambda rbc: [(bounds[i], bounds[i + 1], csr_transpose(A, bounds[i], bounds[i + 1], ks[i], ks[i + 1], pairs=True,  # noqa: E731
-                                                                          col_count=counts[i] if counts else None, rb_counts=rbc,
-                                                                          scratch=scratch))
-                                 for i in range(n_panels) if bounds[i + 1] > bounds[i]]
-            self.panels = build(rb)
-            if rb is not None:
-                if int(scratch["status"][0]) == 0:
-                    self.tiled_fill = True
-                else:          # counts and pattern disagree (the matrix was modified after tfidf): atomic-cursor fill
-                    self.panels = build(None)
+        scratch = {}
+        build = lambda rbc: [(bounds[i], bounds[i + 1], csr_transpose(A, bounds[i], bounds[i + 1], ks[i], ks[i + 1], pairs=True,  # noqa: E731
+                                                                      col_count=counts[i] if counts else None, rb_counts=rbc,
+                                                                      scratch=scratch))
+                             for i in range(n_panels) if bounds[i + 1] > bounds[i]]
+        self.panels = build(rb)
+        if rb is not None:
+            if int(scratch["status"][0]) == 0:
+                self.tiled_fill = True
+            else:          # counts and pattern disagree (the matrix was modified after tfidf): atomic-cursor fill
+                self.panels = build(None)
 
-    def wait(self):
-        if self.ready is not None:
-            torch.cuda.current_stream().wait_event(self.ready)
-            self.ready = None
-
-    def spmm(self, Y: torch.Tensor, dynamic=True, half: bool = False, row_chunks: int = 1, on_chunk=None) -> torch.Tensor:
-        """A^T Y accumulated panel by panel.  ``half``: round Y to IEEE half first (see ``spmm_h16``).
-        ``row_chunks`` > 1 computes the result in that many blocks of output rows (peaks), each finished over all
-        panels before the next starts, and hands every finished block to ``on_chunk`` (the multi-GPU driver starts
-        its allreduce there, under the next block's product)."""
-        self.wait()
+    def spmm(self, Y: torch.Tensor, dynamic=True, half: bool = False) -> torch.Tensor:
+        """A^T Y accumulated panel by panel.  ``half``: round Y to IEEE half first (see ``spmm``)."""
         d, P = self.shape[0], Y.shape[1]
-        Yh = to_half_scaled(Y) if half else None
+        if half:
+            Y = to_half_scaled(Y)
         out = torch.empty((d, P), dtype=torch.float32, device=Y.device)
-        row_chunks = max(1, min(int(row_chunks), d))
-        cuts = [round(i * d / row_chunks) for i in range(row_chunks + 1)]
-        for j0, j1 in zip(cuts[:-1], cuts[1:]):
-            first = True
-            for r0, r1, T in self.panels:
-                if half:
-                    spmm_h16(T, Yh[r0:r1], out=out, accumulate=not first, dynamic=dynamic, rows=(j0, j1))
-                else:
-                    spmm(T, Y[r0:r1], out=out, accumulate=not first, dynamic=dynamic, rows=(j0, j1))
-                first = False
-            if on_chunk is not None:
-                on_chunk(out[j0:j1])
+        for i, (r0, r1, T) in enumerate(self.panels):
+            spmm(T, Y[r0:r1], out=out, accumulate=i > 0, dynamic=dynamic)
         return out
 
     def spmm_rowblocks(self, Y: torch.Tensor, blocks) -> torch.Tensor:
         """Rows ``blocks`` = [(j0, j1), ...] of A^T Y only, stacked into a compact (sum of block heights) x P buffer
         (fp32 operand).  Used for the sampled residual check of the LSI driver: 1/16 of the rows costs 1/16 of a pass."""
-        self.wait()
         P = Y.shape[1]
         total = sum(j1 - j0 for j0, j1 in blocks)
         out = torch.empty((total, P), dtype=torch.float32, device=Y.device)
@@ -633,7 +598,7 @@ class TransposedPanels:
 
 
 def _row_range(rows, n):
-    """``rows`` of spmm / spmm_h16: None = all rows; (j0, j1) = that row range written to the same rows of ``out``;
+    """``rows`` of spmm: None = all rows; (j0, j1) = that row range written to the same rows of ``out``;
     (j0, j1, o0) = written to out rows starting at o0 (a compact buffer of sampled rows)."""
     if rows is None:
         return 0, n, 0
@@ -666,58 +631,26 @@ def to_half_scaled(B: torch.Tensor, scale: float = HALF_SCALE) -> torch.Tensor:
     return out
 
 
-def spmm_h16(A, Bh: torch.Tensor, out: Optional[torch.Tensor] = None, accumulate=False, dynamic=True,
-             scale: float = HALF_SCALE, rows=None) -> torch.Tensor:
-    """C[n x P] (+)= A @ (Bh / scale) with the dense operand stored as IEEE half (``to_half_scaled``): half the
-    bytes per non-zero through the L2 -> L1 gather path that bounds the fp32 kernel; fp32 products and sums."""
-    n, d = A.shape
-    P = Bh.shape[1]
-    assert Bh.shape[0] == d and Bh.dtype == torch.float16 and Bh.is_contiguous(), (Bh.shape, d, Bh.dtype)
-    if out is None:
-        assert not accumulate
-        out = torch.empty((n, P), dtype=torch.float32, device=Bh.device)
-    counter = torch.zeros(1, dtype=torch.int64, device=Bh.device) if dynamic else None
-    j0, j1, o0 = _row_range(rows, n)                    # matrix rows [j0, j1) -> out rows [o0, o0 + j1 - j0)
-    if isinstance(A, DevicePairs):
-        call("mub_spmm_csrp_h16", ptr(A.indptr) + 8 * j0, ptr(A.pairs), j1 - j0, d, ptr(Bh), P, ptr(out) + 4 * P * o0,
-             1 if accumulate else 0, 1.0 / scale, ptr(counter), stream_ptr())
-    else:
-        call("mub_spmm_csr_h16", ptr(A.indptr) + 8 * j0, ptr(A.indices), ptr(A.data), j1 - j0, d, ptr(Bh), P,
-             ptr(out) + 4 * P * o0, 1 if accumulate else 0, 1.0 / scale, ptr(counter), stream_ptr())
-    return out
-
-
-def spmm(A: DeviceCSR, B: torch.Tensor, out: Optional[torch.Tensor] = None, accumulate=False,
-         dynamic=True, algo: Optional[str] = None, rows=None) -> torch.Tensor:
-    """K2/K3: C[n x P] (+)= A @ B[d x P];  P = B.shape[1] must be 32, 64 or 128.
-
-    algo: "rowwarp" (v1: warp per row, B gathered from L2), "panel" (v2: B column panels staged in
-    shared memory by TMA; needs sorted column indices) or None = $MUON_B200_SPMM or auto."""
+def spmm(A, B: torch.Tensor, out: Optional[torch.Tensor] = None, accumulate=False, dynamic=True, rows=None,
+         scale: float = HALF_SCALE) -> torch.Tensor:
+    """K2/K3: C[n x P] (+)= A @ B[d x P];  P = B.shape[1] must be 32, 64 or 128.  A is a ``DeviceCSR`` or
+    ``DevicePairs``.  B is float32, or float16 holding B * ``scale`` (``to_half_scaled``): half the bytes per non-zero
+    through the L2 -> L1 gather path that bounds the fp32 operand; products and sums stay fp32."""
     n, d = A.shape
     P = B.shape[1]
-    assert B.shape[0] == d and B.dtype == torch.float32 and B.is_contiguous(), (B.shape, d, B.dtype)
+    assert B.shape[0] == d and B.dtype in (torch.float32, torch.float16) and B.is_contiguous(), (B.shape, d, B.dtype)
     if out is None:
         assert not accumulate
         out = torch.empty((n, P), dtype=torch.float32, device=B.device)
-    j0, j1, o0 = _row_range(rows, n)                    # matrix rows [j0, j1) -> out rows [o0, o0 + j1 - j0)
-    if isinstance(A, DevicePairs):
-        counter = torch.zeros(1, dtype=torch.int64, device=B.device) if dynamic else None
-        call("mub_spmm_csrp_f32", ptr(A.indptr) + 8 * j0, ptr(A.pairs), j1 - j0, d, ptr(B), P, ptr(out) + 4 * P * o0,
-             1 if accumulate else 0, ptr(counter), stream_ptr())
-        return out
-    if algo is None:
-        algo = os.environ.get("MUON_B200_SPMM", "auto")
-    if algo == "auto":
-        algo = "rowwarp"   # the panel kernel is correct but not yet faster (DESIGN.md section 4)
-    if algo == "panel":
-        if not A.sorted_indices:
-            raise MuonB200Error("spmm(algo='panel') needs sorted column indices")
-        call("mub_spmm_csr_panel_f32", ptr(A.indptr), ptr(A.indices), ptr(A.data), n, d, ptr(B), P, ptr(out),
-             1 if accumulate else 0, stream_ptr())
-        return out
     counter = torch.zeros(1, dtype=torch.int64, device=B.device) if dynamic else None
-    call("mub_spmm_csr_f32", ptr(A.indptr) + 8 * j0, ptr(A.indices), ptr(A.data), j1 - j0, d, ptr(B), P,
-         ptr(out) + 4 * P * o0, 1 if accumulate else 0, ptr(counter), stream_ptr())
+    j0, j1, o0 = _row_range(rows, n)                    # matrix rows [j0, j1) -> out rows [o0, o0 + j1 - j0)
+    pairs = isinstance(A, DevicePairs)
+    operands = [ptr(A.indptr) + 8 * j0] + ([ptr(A.pairs)] if pairs else [ptr(A.indices), ptr(A.data)])
+    operands += [j1 - j0, d, ptr(B), P, ptr(out) + 4 * P * o0, 1 if accumulate else 0]
+    if B.dtype == torch.float16:
+        call("mub_spmm_csrp_h16" if pairs else "mub_spmm_csr_h16", *operands, 1.0 / scale, ptr(counter), stream_ptr())
+    else:
+        call("mub_spmm_csrp_f32" if pairs else "mub_spmm_csr_f32", *operands, ptr(counter), stream_ptr())
     return out
 
 

@@ -28,19 +28,6 @@ def all_reduce_sum_(t: torch.Tensor) -> torch.Tensor:
     return t
 
 
-class _Done:
-    def wait(self):
-        return None
-
-
-def all_reduce_sum_async(t: torch.Tensor):
-    """Sum-allreduce of a contiguous view, in place, without blocking the caller's stream: returns a handle whose
-    ``wait()`` makes the current stream wait for the collective (NCCL runs it on its own stream)."""
-    if is_distributed():
-        return torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.SUM, async_op=True)
-    return _Done()
-
-
 def all_reduce_max_(t: torch.Tensor) -> torch.Tensor:
     if is_distributed():
         torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MAX)

@@ -34,11 +34,9 @@ SIGNATURES = {
     "mub_tfidf_apply_f32": [vp, vp, vp, vp, i64, i32, vp, vp, f32, u32, vp],
     "mub_tfidf_apply_f64": [vp, vp, vp, vp, i64, i32, vp, vp, f64, u32, vp],
     "mub_spmm_csr_f32": [vp, vp, vp, i64, i64, vp, i32, vp, i32, vp, vp],
-    "mub_spmm_csr_panel_f32": [vp, vp, vp, i64, i64, vp, i32, vp, i32, vp],
     "mub_csr_transpose_count": [vp, i64, i32, vp, vp],
     "mub_csr_transpose_fill": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp, vp],
     "mub_gram_f32": [vp, vp, i64, i32, i32, vp, vp, vp],
-    "mub_csr_row_stats_f32": [vp, vp, i64, vp, vp, vp],
     "mub_csr_transpose_fill_pairs": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp],
     "mub_spmm_csrp_f32": [vp, vp, i64, i64, vp, i32, vp, i32, vp, vp],
     "mub_csrp_row_stats_f32": [vp, vp, i64, vp, vp, vp],

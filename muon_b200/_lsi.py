@@ -63,38 +63,24 @@ class CsrOperator:
         self._dev = _device
         self.A = A
         with phase("lsi.transpose"):
-            self.At = A.transpose_panels(pad, side_stream=os.environ.get("MUON_B200_OVERLAP", "0") == "1")
+            self.At = A.transpose_panels(pad)
         self.n_local, self.d = A.shape
         self.n_total = A.n_total
         self.device = A.data.device
         self.passes = 0
 
-    lowp = True      # av / aty accept lowp=True: dense operand rounded to IEEE half (csrc/spmm.cu, spmm_row_h)
+    lowp = True      # av / aty accept lowp=True: dense operand rounded to IEEE half (csrc/spmm.cu)
 
     def av(self, V, lowp: bool = False):
         self.passes += 1
         with phase("lsi.spmm_av"):
-            if lowp:
-                return self._dev.spmm_h16(self.A, self._dev.to_half_scaled(V), dynamic=False)
-            return self._dev.spmm(self.A, V, dynamic=False)
+            return self._dev.spmm(self.A, self._dev.to_half_scaled(V) if lowp else V, dynamic=False)
 
     def aty(self, Y, lowp: bool = False):
-        """A^T Y summed over the cell shards.  Multi-GPU: with $MUON_B200_AR_CHUNKS > 1 the product is computed in
-        blocks of peaks and the allreduce of block c runs (NCCL stream) under the SpMM of block c+1."""
+        """A^T Y summed over the cell shards."""
         self.passes += 1
         with phase("lsi.spmm_aty"):
-            if not _dist.is_distributed():
-                return self.At.spmm(Y, dynamic=True, half=lowp)
-            works = []
-            W = self.At.spmm(Y, dynamic=True, half=lowp, row_chunks=self.AR_CHUNKS,
-                             on_chunk=lambda blk: works.append(_dist.all_reduce_sum_async(blk)))
-            for w in works:
-                w.wait()
-            return W
-
-    # several blocks overlap the allreduce with the product but split the SpMM into smaller, less efficient
-    # launches, and the allreduce of a d x P block is short, so the default is one block (the overlapped path stays available and tested)
-    AR_CHUNKS = int(os.environ.get("MUON_B200_AR_CHUNKS", "1"))
+            return _dist.all_reduce_sum_(self.At.spmm(Y, dynamic=True, half=lowp))
 
     def residual_sample(self, Uk, Vk, sig):
         """Estimate of the relative residuals ||A^T u_i - sigma_i v_i|| / sigma_i of k triplets from 1/16 of the

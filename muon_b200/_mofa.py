@@ -66,13 +66,9 @@ class _Block:
     def moments(self, D, dev):
         """per-feature sum and sum of squares over the block's cells (fp64), from the transposed panels"""
         s1, s2 = torch.zeros(D, dtype=f64, device=dev), torch.zeros(D, dtype=f64, device=dev)
-        self.At.wait()
         for (_, _, T) in self.At.panels:
             t1, t2 = torch.empty(D, dtype=f64, device=dev), torch.empty(D, dtype=f64, device=dev)
-            if isinstance(T, _device.DevicePairs):
-                call("mub_csrp_row_stats_f32", ptr(T.indptr), ptr(T.pairs), D, ptr(t1), ptr(t2), stream_ptr())
-            else:
-                call("mub_csr_row_stats_f32", ptr(T.indptr), ptr(T.data), D, ptr(t1), ptr(t2), stream_ptr())
+            call("mub_csrp_row_stats_f32", ptr(T.indptr), ptr(T.pairs), D, ptr(t1), ptr(t2), stream_ptr())
             s1 += t1
             s2 += t2
         return s1, s2
@@ -152,7 +148,6 @@ class _SparsePseudoBlock:
         ssq = torch.empty(D, dtype=f64, device=C.device)
         call("mub_mofa_lowrank_cols_f32", ptr(self.Zz), n, ptr(self.Wz), D, ptr(self.kappa), ptr(C), self.ld, self.kind,
              ptr(P), ptr(ssq), st)
-        self.At.wait()
         row = 4 * self.ld
         for r0, _, T in self.At.panels:
             call("mub_mofa_nnz_cols_f32", ptr(T.indptr), ptr(T.pairs), D, ptr(self.Zz) + row * r0, ptr(self.Wz),

@@ -6,16 +6,24 @@
 // contractions (muon/_core/tools.py:583-585).  A^T * Y uses the same kernel on the CSR of
 // A^T (transpose.cu).
 //
-// v1 "row-warp" kernel: a warp owns a row.  Lane layout: P/4 lanes cover one dense row as
-// float4 (16 B per lane, 4P bytes per non-zero, fully coalesced), so a warp consumes
-// G = 128/P non-zeros per gather instruction.  Column indices and values are streamed in
-// coalesced 128 B segments (32 per warp load, L1::no_allocate) and broadcast by shuffle;
-// 32/G independent float4 gathers are in flight per lane.  fp32 FMA accumulation in
-// registers, one float4 store per lane group at the end of the row.
+// "Row-warp" kernel: a warp owns a row.  The dense operand B is fp32 or IEEE half (T).  Every lane
+// gathers 16 B of a row of B, VEC = 16 / sizeof(T) values, so P/VEC lanes cover one row and a warp
+// consumes G = 32 / (P/VEC) non-zeros per gather instruction.  Column indices and values are streamed
+// in coalesced 128 B segments (32 per warp load, L1::no_allocate) and broadcast by shuffle; up to 16
+// independent gathers are in flight per lane.  fp32 FMA accumulation in registers, 16 B stores per
+// lane at the end of the row.
 //
 // Traffic model (DESIGN.md): HBM streams 8 B/nnz (+ dense operands once); every non-zero
-// additionally pulls 4P bytes of B through L2->L1, which is the practical limiter at P>=32.
+// additionally pulls P * sizeof(T) bytes of B through L2->L1, which is the practical limiter at P>=32.
+//
+// Half operand: every non-zero gathers half the bytes of the fp32 kernel.  Products and sums are fp32
+// (half -> float conversion is exact), only the operand is rounded (2^-11 relative).  Used by the early
+// block-Lanczos steps of the LSI driver (_lsi.py), whose accuracy need not exceed 1e-3; the final steps
+// use the fp32 operand.  out_scale undoes the power-of-two scaling the caller applied before rounding
+// (mub_f32_to_f16_scaled).
 #include <cuda_fp16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -38,19 +46,40 @@ __device__ __forceinline__ void load_entry(const int32_t* __restrict__ indices, 
     }
 }
 
-template <int P, bool PAIRS>
+// acc[i] += v * (i-th value of the 16 B gather q)
+template <typename T>
+__device__ __forceinline__ void fma_gather(float* acc, float v, const uint4& q) {
+    const unsigned w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        if constexpr (std::is_same_v<T, float>) {
+            acc[i] = fmaf(v, __uint_as_float(w[i]), acc[i]);
+        } else {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+            acc[2 * i] = fmaf(v, f.x, acc[2 * i]);
+            acc[2 * i + 1] = fmaf(v, f.y, acc[2 * i + 1]);
+        }
+    }
+}
+
+template <int P, bool PAIRS, typename T>
 __device__ __forceinline__ void spmm_row(const int32_t* __restrict__ indices, const float* __restrict__ data,
-                                         int64_t start, int64_t end, const float* __restrict__ B,
-                                         float* __restrict__ C_row, int accumulate, int lane) {
-    constexpr int LPN = P / 4;    // lanes per non-zero
-    constexpr int G = 32 / LPN;   // non-zeros per warp-wide gather
-    constexpr int STEPS = 32 / G; // gathers per 32-nnz segment
+                                         int64_t start, int64_t end, const T* __restrict__ B,
+                                         float* __restrict__ C_row, int accumulate, float out_scale, int lane) {
+    constexpr int VEC = 16 / sizeof(T);            // values per 16 B gather
+    constexpr int LPN = P / VEC;                   // lanes per non-zero
+    constexpr int G = 32 / LPN;                    // non-zeros per warp-wide gather
+    constexpr int STEPS = 32 / G;                  // gathers per 32-nnz segment
+    constexpr int BATCH = STEPS < 16 ? STEPS : 16; // gathers in flight per lane
     const int sub = lane % LPN, grp = lane / LPN;
-    const float* Bl = B + sub * 4;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    const T* Bl = B + sub * VEC;
+    float acc[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
     int64_t base = start;
-    // full 32-nnz segments: all STEPS gathers issued back to back; the next segment's (index, value) entries are
-    // requested from HBM before the gathers of the current one (see spmm_row_h)
+    // full 32-nnz segments.  The (index, value) stream comes from HBM (~600 ns), the gathers from L2 (~130 ns):
+    // the NEXT segment's entries are requested before the gathers of the current one, so a warp never waits for
+    // both latencies in sequence
     int c_next = 0;
     float v_next = 0.f;
     bool more = base + 32 <= end;
@@ -60,24 +89,18 @@ __device__ __forceinline__ void spmm_row(const int32_t* __restrict__ indices, co
         const float v = v_next;
         more = base + 64 <= end;
         if (more) load_entry<PAIRS>(indices, data, base + 32 + lane, c_next, v_next);
-        constexpr int BATCH = STEPS < 16 ? STEPS : 16;  // gathers in flight per lane
 #pragma unroll
         for (int t0 = 0; t0 < STEPS; t0 += BATCH) {
-            float4 b[BATCH];
+            uint4 b[BATCH];
             float vv[BATCH];
 #pragma unroll
             for (int t = 0; t < BATCH; ++t) {
                 const int cc = __shfl_sync(0xffffffffu, c, (t0 + t) * G + grp);
                 vv[t] = __shfl_sync(0xffffffffu, v, (t0 + t) * G + grp);
-                b[t] = ld_gather4(Bl + (size_t)cc * P);
+                b[t] = ld_gather_u4(Bl + (size_t)cc * P);
             }
 #pragma unroll
-            for (int t = 0; t < BATCH; ++t) {
-                acc.x = fmaf(vv[t], b[t].x, acc.x);
-                acc.y = fmaf(vv[t], b[t].y, acc.y);
-                acc.z = fmaf(vv[t], b[t].z, acc.z);
-                acc.w = fmaf(vv[t], b[t].w, acc.w);
-            }
+            for (int t = 0; t < BATCH; ++t) fma_gather<T>(acc, vv[t], b[t]);
         }
     }
     if (base < end) {  // tail segment (warp-uniform trip count)
@@ -88,48 +111,50 @@ __device__ __forceinline__ void spmm_row(const int32_t* __restrict__ indices, co
         if (ok) load_entry<PAIRS>(indices, data, base + lane, c, v);
         const int steps = (cnt + G - 1) / G;
         for (int t = 0; t < steps; ++t) {
-            const int src = t * G + grp;
+            const int src = t * G + grp;  // < 32: G divides 32 and cnt < 32
             const int cc = __shfl_sync(0xffffffffu, c, src);
             const float vt = __shfl_sync(0xffffffffu, v, src);
-            if (src < cnt) {
-                const float4 bt = ld_gather4(Bl + (size_t)cc * P);
-                acc.x = fmaf(vt, bt.x, acc.x);
-                acc.y = fmaf(vt, bt.y, acc.y);
-                acc.z = fmaf(vt, bt.z, acc.z);
-                acc.w = fmaf(vt, bt.w, acc.w);
-            }
+            if (src < cnt) fma_gather<T>(acc, vt, ld_gather_u4(Bl + (size_t)cc * P));
         }
     }
     // combine the G lane groups (fixed butterfly order: deterministic)
 #pragma unroll
     for (int off = LPN; off < 32; off <<= 1) {
-        acc.x += __shfl_xor_sync(0xffffffffu, acc.x, off);
-        acc.y += __shfl_xor_sync(0xffffffffu, acc.y, off);
-        acc.z += __shfl_xor_sync(0xffffffffu, acc.z, off);
-        acc.w += __shfl_xor_sync(0xffffffffu, acc.w, off);
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
     }
     if (grp == 0) {
-        float4* dst = reinterpret_cast<float4*>(C_row + sub * 4);
-        if (accumulate) {
-            const float4 o = *dst;
-            acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
+        float4* dst = reinterpret_cast<float4*>(C_row + sub * VEC);
+#pragma unroll
+        for (int j = 0; j < VEC / 4; ++j) {
+            float4 r = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+            if constexpr (std::is_same_v<T, __half>) {
+                // __fmul_rn is never contracted with the add below: the scaled product is rounded on its own, as it
+                // is without accumulate
+                r.x = __fmul_rn(r.x, out_scale); r.y = __fmul_rn(r.y, out_scale);
+                r.z = __fmul_rn(r.z, out_scale); r.w = __fmul_rn(r.w, out_scale);
+            }
+            if (accumulate) {
+                const float4 o = dst[j];
+                r.x += o.x; r.y += o.y; r.z += o.z; r.w += o.w;
+            }
+            dst[j] = r;
         }
-        *dst = acc;
     }
 }
 
-template <int P, bool PAIRS>
+template <int P, bool PAIRS, typename T>
 __global__ void __launch_bounds__(kSpmmThreads)
 spmm_csr_rowwarp_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                        const float* __restrict__ data, int64_t n_rows, const float* __restrict__ B,
-                        float* __restrict__ C, int accumulate, unsigned long long* row_counter) {
+                        const float* __restrict__ data, int64_t n_rows, const T* __restrict__ B,
+                        float* __restrict__ C, int accumulate, float out_scale, unsigned long long* row_counter) {
     const int lane = threadIdx.x & 31;
     if (row_counter == nullptr) {
         const int64_t warp = (int64_t)blockIdx.x * kSpmmWarps + (threadIdx.x >> 5);
         const int64_t n_warps = (int64_t)gridDim.x * kSpmmWarps;
         for (int64_t row = warp; row < n_rows; row += n_warps) {
             const int64_t s = __ldg(indptr + row), e = __ldg(indptr + row + 1);
-            spmm_row<P, PAIRS>(indices, data, s, e, B, C + (size_t)row * P, accumulate, lane);
+            spmm_row<P, PAIRS, T>(indices, data, s, e, B, C + (size_t)row * P, accumulate, out_scale, lane);
         }
     } else {
         // dynamic scheduling: each warp claims the next unprocessed row (rows are issued in
@@ -140,131 +165,42 @@ spmm_csr_rowwarp_kernel(const int64_t* __restrict__ indptr, const int32_t* __res
             row = __shfl_sync(0xffffffffu, row, 0);
             if ((int64_t)row >= n_rows) break;
             const int64_t s = __ldg(indptr + row), e = __ldg(indptr + row + 1);
-            spmm_row<P, PAIRS>(indices, data, s, e, B, C + (size_t)row * P, accumulate, lane);
+            spmm_row<P, PAIRS, T>(indices, data, s, e, B, C + (size_t)row * P, accumulate, out_scale, lane);
         }
     }
 }
 
-// ---- half-precision dense operand -------------------------------------------------------------------
-// Same row-warp product with B stored as IEEE half (row = 2P bytes): every non-zero gathers half the bytes
-// through L2 -> L1 -> registers, which is what bounds the fp32 kernel (DESIGN.md section 4).  Products and
-// sums are fp32 (half -> float conversion is exact), only the operand is rounded (2^-11 relative).  Used
-// by the early block-Lanczos steps of the LSI driver (_lsi.py), whose accuracy need not exceed 1e-3;
-// the final steps run the fp32 kernel above.  Lane layout: P/8 lanes cover one row of B (16 B = 8 halves
-// per lane), a warp consumes G = 256/P non-zeros per gather instruction.  out_scale undoes the power-of-
-// two scaling the caller applied before rounding (mub_f32_to_f16_scaled).
-template <int P, bool PAIRS>
-__device__ __forceinline__ void spmm_row_h(const int32_t* __restrict__ indices, const float* __restrict__ data,
-                                           int64_t start, int64_t end, const __half* __restrict__ B,
-                                           float* __restrict__ C_row, int accumulate, float out_scale, int lane) {
-    constexpr int LPN = P / 8;      // lanes per non-zero
-    constexpr int G = 32 / LPN;     // non-zeros per warp-wide gather
-    constexpr int STEPS = 32 / G;   // gathers per 32-nnz segment
-    const int sub = lane % LPN, grp = lane / LPN;
-    const __half* Bl = B + sub * 8;
-    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    auto fma8 = [&](float v, const uint4& q) {
-        const unsigned w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-            acc[2 * i] = fmaf(v, f.x, acc[2 * i]);
-            acc[2 * i + 1] = fmaf(v, f.y, acc[2 * i + 1]);
-        }
-    };
-    int64_t base = start;
-    // the (index, value) stream comes from HBM (~600 ns), the gathers from L2 (~130 ns): fetch the NEXT segment's
-    // entries before gathering for the current one, so a warp never waits for both latencies in sequence
-    int c_next = 0;
-    float v_next = 0.f;
-    bool more = base + 32 <= end;
-    if (more) load_entry<PAIRS>(indices, data, base + lane, c_next, v_next);
-    while (more) {
-        const int c = c_next;
-        const float v = v_next;
-        more = base + 64 <= end;
-        if (more) load_entry<PAIRS>(indices, data, base + 32 + lane, c_next, v_next);
-        uint4 b[STEPS];
-        float vv[STEPS];
-#pragma unroll
-        for (int t = 0; t < STEPS; ++t) {
-            const int cc = __shfl_sync(0xffffffffu, c, t * G + grp);
-            vv[t] = __shfl_sync(0xffffffffu, v, t * G + grp);
-            b[t] = ld_gather_u4(Bl + (size_t)cc * P);
-        }
-#pragma unroll
-        for (int t = 0; t < STEPS; ++t) fma8(vv[t], b[t]);
-        base += 32;
-    }
-    if (base < end) {
-        const int cnt = (int)(end - base);
-        const bool ok = lane < cnt;
-        int c = 0;
-        float v = 0.f;
-        if (ok) load_entry<PAIRS>(indices, data, base + lane, c, v);
-        const int steps = (cnt + G - 1) / G;
-        for (int t = 0; t < steps; ++t) {
-            const int src = t * G + grp;
-            const int cc = __shfl_sync(0xffffffffu, c, src & 31);
-            const float vt = __shfl_sync(0xffffffffu, v, src & 31);
-            if (src < cnt) fma8(vt, ld_gather_u4(Bl + (size_t)cc * P));
-        }
-    }
-#pragma unroll
-    for (int off = LPN; off < 32; off <<= 1) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
-    }
-    if (grp == 0) {
-        float4* dst = reinterpret_cast<float4*>(C_row + sub * 8);
-        float4 lo = make_float4(acc[0] * out_scale, acc[1] * out_scale, acc[2] * out_scale, acc[3] * out_scale);
-        float4 hi = make_float4(acc[4] * out_scale, acc[5] * out_scale, acc[6] * out_scale, acc[7] * out_scale);
-        if (accumulate) {
-            const float4 o0 = dst[0], o1 = dst[1];
-            lo.x += o0.x; lo.y += o0.y; lo.z += o0.z; lo.w += o0.w;
-            hi.x += o1.x; hi.y += o1.y; hi.z += o1.z; hi.w += o1.w;
-        }
-        dst[0] = lo;
-        dst[1] = hi;
-    }
-}
-
-template <int P, bool PAIRS>
-__global__ void __launch_bounds__(kSpmmThreads)
-spmm_csr_rowwarp_h_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                          const float* __restrict__ data, int64_t n_rows, const __half* __restrict__ B,
-                          float* __restrict__ C, int accumulate, float out_scale, unsigned long long* row_counter) {
-    const int lane = threadIdx.x & 31;
-    if (row_counter == nullptr) {
-        const int64_t warp = (int64_t)blockIdx.x * kSpmmWarps + (threadIdx.x >> 5);
-        const int64_t n_warps = (int64_t)gridDim.x * kSpmmWarps;
-        for (int64_t row = warp; row < n_rows; row += n_warps) {
-            const int64_t s = __ldg(indptr + row), e = __ldg(indptr + row + 1);
-            spmm_row_h<P, PAIRS>(indices, data, s, e, B, C + (size_t)row * P, accumulate, out_scale, lane);
-        }
-    } else {
-        for (;;) {
-            unsigned long long row = 0;
-            if (lane == 0) row = atomicAdd(row_counter, 1ull);
-            row = __shfl_sync(0xffffffffu, row, 0);
-            if ((int64_t)row >= n_rows) break;
-            const int64_t s = __ldg(indptr + row), e = __ldg(indptr + row + 1);
-            spmm_row_h<P, PAIRS>(indices, data, s, e, B, C + (size_t)row * P, accumulate, out_scale, lane);
-        }
-    }
-}
-
-template <int P, bool PAIRS>
-static int launch_spmm_h(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
-                         const __half* B, float* C, int accumulate, float out_scale, unsigned long long* row_counter,
-                         cudaStream_t stream) {
+template <int P, bool PAIRS, typename T>
+static int launch_spmm(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
+                       const T* B, float* C, int accumulate, float out_scale, unsigned long long* row_counter,
+                       cudaStream_t stream, const char* name) {
     int64_t want = (n_rows + kSpmmWarps - 1) / kSpmmWarps;
-    int64_t cap = (int64_t)sm_count() * 8;
+    int64_t cap = (int64_t)sm_count() * 8;  // 2048 threads / SM
     int grid = (int)(want < cap ? want : cap);
     if (grid < 1) grid = 1;
-    spmm_csr_rowwarp_h_kernel<P, PAIRS><<<grid, kSpmmThreads, 0, stream>>>(indptr, indices, data, n_rows, B, C,
-                                                                     accumulate, out_scale, row_counter);
-    return check_launch("spmm_csr_h16");
+    spmm_csr_rowwarp_kernel<P, PAIRS, T><<<grid, kSpmmThreads, 0, stream>>>(indptr, indices, data, n_rows, B, C,
+                                                                          accumulate, out_scale, row_counter);
+    return check_launch(name);
+}
+
+// the four C entry points: shared validation, then one instantiation per ld
+template <bool PAIRS, typename T>
+static int spmm_entry(const char* name, const int64_t* indptr, const int32_t* indices, const float* data,
+                      int64_t n_rows, int64_t n_cols, const void* B, int32_t ld, float* C, int32_t accumulate,
+                      float out_scale, unsigned long long* row_counter, mub_stream_t stream) {
+    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "%s: negative shape", name);
+    MUB_REQUIRE(ld == 32 || ld == 64 || ld == 128, "%s: ld must be 32, 64 or 128 (got %d)", name, ld);
+    if (n_rows == 0) return 0;
+    MUB_REQUIRE(indptr && B && C, "%s: null pointer", name);
+    MUB_REQUIRE((((uintptr_t)B | (uintptr_t)C) & 15) == 0, "%s: B and C must be 16-byte aligned", name);
+    MUB_REQUIRE(!PAIRS || ((uintptr_t)indices & 7) == 0, "%s: pairs must be 8-byte aligned", name);
+    const T* Bt = (const T*)B;
+    cudaStream_t s = (cudaStream_t)stream;
+    switch (ld) {
+        case 32: return launch_spmm<32, PAIRS, T>(indptr, indices, data, n_rows, Bt, C, accumulate, out_scale, row_counter, s, name);
+        case 64: return launch_spmm<64, PAIRS, T>(indptr, indices, data, n_rows, Bt, C, accumulate, out_scale, row_counter, s, name);
+        default: return launch_spmm<128, PAIRS, T>(indptr, indices, data, n_rows, Bt, C, accumulate, out_scale, row_counter, s, name);
+    }
 }
 
 // dst[i] = half(src[i] * scale): the rounding step in front of the half-operand products
@@ -282,54 +218,36 @@ f32_to_f16_scaled_kernel(const float4* __restrict__ src, int64_t n4, float scale
     }
 }
 
-template <int P, bool PAIRS>
-static int launch_spmm(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
-                       const float* B, float* C, int accumulate, unsigned long long* row_counter,
-                       cudaStream_t stream) {
-    int64_t want = (n_rows + kSpmmWarps - 1) / kSpmmWarps;
-    int64_t cap = (int64_t)sm_count() * 8;  // 2048 threads / SM
-    int grid = (int)(want < cap ? want : cap);
-    if (grid < 1) grid = 1;
-    spmm_csr_rowwarp_kernel<P, PAIRS><<<grid, kSpmmThreads, 0, stream>>>(indptr, indices, data, n_rows, B, C,
-                                                                   accumulate, row_counter);
-    return check_launch("spmm_csr");
-}
-
 }  // namespace mub
 
 extern "C" int mub_spmm_csr_f32(const int64_t* indptr, const int32_t* indices, const float* data,
                                 int64_t n_rows, int64_t n_cols, const float* B, int32_t ld, float* C,
                                 int32_t accumulate, unsigned long long* row_counter, mub_stream_t stream) {
-    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "spmm_csr: negative shape");
-    MUB_REQUIRE(ld == 32 || ld == 64 || ld == 128, "spmm_csr: ld must be 32, 64 or 128 (got %d)", ld);
-    if (n_rows == 0) return 0;
-    MUB_REQUIRE(indptr && B && C, "spmm_csr: null pointer");
-    MUB_REQUIRE((((uintptr_t)B | (uintptr_t)C) & 15) == 0, "spmm_csr: B and C must be 16-byte aligned");
-    cudaStream_t s = (cudaStream_t)stream;
-    switch (ld) {
-        case 32: return mub::launch_spmm<32, false>(indptr, indices, data, n_rows, B, C, accumulate, row_counter, s);
-        case 64: return mub::launch_spmm<64, false>(indptr, indices, data, n_rows, B, C, accumulate, row_counter, s);
-        default: return mub::launch_spmm<128, false>(indptr, indices, data, n_rows, B, C, accumulate, row_counter, s);
-    }
+    return mub::spmm_entry<false, float>("spmm_csr", indptr, indices, data, n_rows, n_cols, B, ld, C, accumulate, 1.f,
+                                         row_counter, stream);
 }
 
 extern "C" int mub_spmm_csrp_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, int64_t n_cols,
                                  const float* B, int32_t ld, float* C, int32_t accumulate,
                                  unsigned long long* row_counter, mub_stream_t stream) {
-    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "spmm_csrp: negative shape");
-    MUB_REQUIRE(ld == 32 || ld == 64 || ld == 128, "spmm_csrp: ld must be 32, 64 or 128 (got %d)", ld);
-    if (n_rows == 0) return 0;
-    MUB_REQUIRE(indptr && B && C, "spmm_csrp: null pointer");
-    MUB_REQUIRE((((uintptr_t)B | (uintptr_t)C) & 15) == 0 && ((uintptr_t)pairs & 7) == 0, "spmm_csrp: misaligned operand");
-    cudaStream_t s = (cudaStream_t)stream;
-    switch (ld) {
-        case 32: return mub::launch_spmm<32, true>(indptr, pairs, nullptr, n_rows, B, C, accumulate, row_counter, s);
-        case 64: return mub::launch_spmm<64, true>(indptr, pairs, nullptr, n_rows, B, C, accumulate, row_counter, s);
-        default: return mub::launch_spmm<128, true>(indptr, pairs, nullptr, n_rows, B, C, accumulate, row_counter, s);
-    }
+    return mub::spmm_entry<true, float>("spmm_csrp", indptr, pairs, nullptr, n_rows, n_cols, B, ld, C, accumulate, 1.f,
+                                        row_counter, stream);
 }
 
-// ---- half-precision dense operand (see spmm_row_h) ---------------------------------------------------
+extern "C" int mub_spmm_csr_h16(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
+                                int64_t n_cols, const void* B_half, int32_t ld, float* C, int32_t accumulate,
+                                float out_scale, unsigned long long* row_counter, mub_stream_t stream) {
+    return mub::spmm_entry<false, __half>("spmm_csr_h16", indptr, indices, data, n_rows, n_cols, B_half, ld, C,
+                                          accumulate, out_scale, row_counter, stream);
+}
+
+extern "C" int mub_spmm_csrp_h16(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, int64_t n_cols,
+                                 const void* B_half, int32_t ld, float* C, int32_t accumulate, float out_scale,
+                                 unsigned long long* row_counter, mub_stream_t stream) {
+    return mub::spmm_entry<true, __half>("spmm_csrp_h16", indptr, pairs, nullptr, n_rows, n_cols, B_half, ld, C,
+                                         accumulate, out_scale, row_counter, stream);
+}
+
 extern "C" int mub_f32_to_f16_scaled(const float* src, int64_t n, float scale, void* dst, mub_stream_t stream) {
     MUB_REQUIRE(n >= 0 && (n % 4) == 0, "f32_to_f16_scaled: n must be a non-negative multiple of 4");
     if (n == 0) return 0;
@@ -338,38 +256,4 @@ extern "C" int mub_f32_to_f16_scaled(const float* src, int64_t n, float scale, v
     int grid = (int)(want < cap ? want : cap);
     mub::f32_to_f16_scaled_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float4*)src, n / 4, scale, (uint2*)dst);
     return mub::check_launch("f32_to_f16_scaled");
-}
-
-extern "C" int mub_spmm_csr_h16(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
-                                int64_t n_cols, const void* B_half, int32_t ld, float* C, int32_t accumulate,
-                                float out_scale, unsigned long long* row_counter, mub_stream_t stream) {
-    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "spmm_csr_h16: negative shape");
-    MUB_REQUIRE(ld == 32 || ld == 64 || ld == 128, "spmm_csr_h16: ld must be 32, 64 or 128 (got %d)", ld);
-    if (n_rows == 0) return 0;
-    MUB_REQUIRE(indptr && B_half && C, "spmm_csr_h16: null pointer");
-    MUB_REQUIRE((((uintptr_t)B_half | (uintptr_t)C) & 15) == 0, "spmm_csr_h16: B and C must be 16-byte aligned");
-    cudaStream_t s = (cudaStream_t)stream;
-    const __half* B = (const __half*)B_half;
-    switch (ld) {
-        case 32: return mub::launch_spmm_h<32, false>(indptr, indices, data, n_rows, B, C, accumulate, out_scale, row_counter, s);
-        case 64: return mub::launch_spmm_h<64, false>(indptr, indices, data, n_rows, B, C, accumulate, out_scale, row_counter, s);
-        default: return mub::launch_spmm_h<128, false>(indptr, indices, data, n_rows, B, C, accumulate, out_scale, row_counter, s);
-    }
-}
-
-extern "C" int mub_spmm_csrp_h16(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, int64_t n_cols,
-                                 const void* B_half, int32_t ld, float* C, int32_t accumulate, float out_scale,
-                                 unsigned long long* row_counter, mub_stream_t stream) {
-    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "spmm_csrp_h16: negative shape");
-    MUB_REQUIRE(ld == 32 || ld == 64 || ld == 128, "spmm_csrp_h16: ld must be 32, 64 or 128 (got %d)", ld);
-    if (n_rows == 0) return 0;
-    MUB_REQUIRE(indptr && B_half && C, "spmm_csrp_h16: null pointer");
-    MUB_REQUIRE((((uintptr_t)B_half | (uintptr_t)C) & 15) == 0 && ((uintptr_t)pairs & 7) == 0, "spmm_csrp_h16: misaligned operand");
-    cudaStream_t s = (cudaStream_t)stream;
-    const __half* B = (const __half*)B_half;
-    switch (ld) {
-        case 32: return mub::launch_spmm_h<32, true>(indptr, pairs, nullptr, n_rows, B, C, accumulate, out_scale, row_counter, s);
-        case 64: return mub::launch_spmm_h<64, true>(indptr, pairs, nullptr, n_rows, B, C, accumulate, out_scale, row_counter, s);
-        default: return mub::launch_spmm_h<128, true>(indptr, pairs, nullptr, n_rows, B, C, accumulate, out_scale, row_counter, s);
-    }
 }

@@ -335,6 +335,8 @@ transpose_fill_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* _
     if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(status, 1);
 }
 
+// per-row sum and sum of squares (fp64 accumulation); applied to the transposed panels of A this yields
+// the per-feature moments MOFA's centring needs (intercepts, muon/_core/tools.py:283-286)
 __global__ void __launch_bounds__(256)
 row_stats_pairs_kernel(const int64_t* __restrict__ indptr, const int2* __restrict__ pairs, int64_t n_rows,
                        double* __restrict__ sum, double* __restrict__ sumsq) {
@@ -346,31 +348,6 @@ row_stats_pairs_kernel(const int64_t* __restrict__ indptr, const int2* __restric
         double a = 0.0, b = 0.0;
         for (int64_t k = s + lane; k < e; k += 32) {
             const double v = (double)__int_as_float(ld_stream2(pairs + k).y);
-            a += v;
-            b += v * v;
-        }
-        a = warp_sum(a);
-        b = warp_sum(b);
-        if (lane == 0) {
-            sum[row] = a;
-            sumsq[row] = b;
-        }
-    }
-}
-
-// per-row sum and sum of squares (fp64 accumulation); applied to the CSR of A^T this yields
-// the per-feature moments MOFA's centring needs (intercepts, muon/_core/tools.py:283-286)
-__global__ void __launch_bounds__(256)
-row_stats_kernel(const int64_t* __restrict__ indptr, const float* __restrict__ data, int64_t n_rows,
-                 double* __restrict__ sum, double* __restrict__ sumsq) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
-    const int64_t n_warps = (int64_t)gridDim.x * 8;
-    for (int64_t row = warp; row < n_rows; row += n_warps) {
-        const int64_t s = __ldg(indptr + row), e = __ldg(indptr + row + 1);
-        double a = 0.0, b = 0.0;
-        for (int64_t k = s + lane; k < e; k += 32) {
-            const double v = (double)ld_stream(data + k);
             a += v;
             b += v * v;
         }
@@ -415,17 +392,6 @@ int mub_csrp_row_stats_f32(const int64_t* indptr, const int32_t* pairs, int64_t 
     mub::row_stats_pairs_kernel<<<grid < 1 ? 1 : grid, 256, 0, (cudaStream_t)stream>>>(indptr, (const int2*)pairs,
                                                                                      n_rows, sum, sumsq);
     return mub::check_launch("csrp_row_stats");
-}
-
-int mub_csr_row_stats_f32(const int64_t* indptr, const float* data, int64_t n_rows, double* sum, double* sumsq,
-                          mub_stream_t stream) {
-    MUB_REQUIRE(n_rows >= 0, "csr_row_stats: negative n_rows");
-    if (n_rows == 0) return 0;
-    MUB_REQUIRE(indptr && sum && sumsq, "csr_row_stats: null pointer");
-    int64_t want = (n_rows + 7) / 8, cap = (int64_t)mub::sm_count() * 8;
-    int grid = (int)(want < cap ? want : cap);
-    mub::row_stats_kernel<<<grid < 1 ? 1 : grid, 256, 0, (cudaStream_t)stream>>>(indptr, data, n_rows, sum, sumsq);
-    return mub::check_launch("csr_row_stats");
 }
 
 int mub_csr_transpose_count(const int32_t* indices, int64_t nnz, int32_t n_cols, int64_t* t_count,

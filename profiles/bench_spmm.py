@@ -1,5 +1,9 @@
-"""Micro-benchmark of the SpMM kernels (v1 row-warp vs v2 TMA panel) on a slice of the bench matrix.
-    python profiles/bench_spmm.py [cells] [peaks] [P]"""
+"""Micro-benchmark of the four row-warp SpMM entry points on a slice of the bench matrix: A·B on the CSR arrays
+(mub_spmm_csr_*) and Aᵀ·B on the transposed pairs panels (mub_spmm_csrp_*), fp32 and half operand, P = 32, 64, 128.
+CUDA events around `reps` passes after `warmup` passes; the digest of each output lets two library builds
+(MUON_B200_LIB) be compared bit for bit.
+    python profiles/bench_spmm.py [cells] [peaks] [reps]"""
+import hashlib
 import os
 import sys
 
@@ -11,23 +15,40 @@ from muon_b200._synth import generate_device, make_tables  # noqa: E402
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 100_000
 d = int(sys.argv[2]) if len(sys.argv) > 2 else 200_000
-P = int(sys.argv[3]) if len(sys.argv) > 3 else 64
-A = generate_device(n, d, 0.03, tables=make_tables(d, 0.03, 64, 1))
-B = torch.randn((d, P), device="cuda")
-ref = None
-for algo in ("rowwarp", "panel"):
-    for _ in range(10):   # warm up clocks and caches
-        C = _device.spmm(A, B, algo=algo, dynamic=False)
-    torch.cuda.synchronize()
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-    ev[0].record()
-    for _ in range(10):
-        C = _device.spmm(A, B, algo=algo, dynamic=False)
-    ev[1].record()
-    torch.cuda.synchronize()
-    ms = ev[0].elapsed_time(ev[1]) / 10
-    gb = (8 * A.nnz + 4 * P * (n + d)) / 1e9
-    err = 0.0 if ref is None else float((C - ref).abs().max() / ref.abs().max())
-    ref = C if ref is None else ref
-    print(f"{algo:8s} n={n} d={d} P={P} nnz={A.nnz}: {ms:.3f} ms  {gb / ms * 1e3:.0f} GB/s algorithmic  "
-          f"{ms * 1e9 / A.nnz:.1f} ps/nnz  maxrel diff vs v1 {err:.2e}")
+reps = int(sys.argv[3]) if len(sys.argv) > 3 else 10
+warmup = 3
+A = _device.tfidf_csr(generate_device(n, d, 0.03, tables=make_tables(d, 0.03, 64, 1)))
+g = torch.Generator(device="cuda").manual_seed(0)
+
+
+def csr_pass(B):
+    return _device.spmm(A, B, dynamic=False)
+
+
+def pairs_pass(B):
+    out = torch.empty((d, B.shape[1]), dtype=torch.float32, device=B.device)
+    for i, (r0, r1, T) in enumerate(At.panels):
+        _device.spmm(T, B[r0:r1], out=out, accumulate=i > 0, dynamic=True)
+    return out
+
+
+print(f"n={n} d={d} nnz={A.nnz} reps={reps} {torch.cuda.get_device_name()}")
+for P in (32, 64, 128):
+    At = A.transpose_panels(P)
+    for name, run, rows in (("csr", csr_pass, d), ("csrp", pairs_pass, n)):
+        B32 = torch.randn((rows, P), generator=g, device="cuda") / 30.0
+        for dtype, B in (("f32", B32), ("h16", _device.to_half_scaled(B32))):
+            for _ in range(warmup):
+                C = run(B)
+            torch.cuda.synchronize()
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+            ev[0].record()
+            for _ in range(reps):
+                C = run(B)
+            ev[1].record()
+            torch.cuda.synchronize()
+            ms = ev[0].elapsed_time(ev[1]) / reps
+            gb = (8 * A.nnz + B.element_size() * P * (n + d)) / 1e9
+            digest = hashlib.sha256(C.cpu().numpy().tobytes()).hexdigest()[:16]
+            print(f"mub_spmm_{name}_{dtype} P={P:3d}: {ms:8.3f} ms  {gb / ms * 1e3:5.0f} GB/s algorithmic  "
+                  f"{ms * 1e9 / A.nnz:5.1f} ps/nnz  digest {digest}")

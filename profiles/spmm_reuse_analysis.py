@@ -55,8 +55,8 @@ out["reading"] = ("83 % of the non-zeros come from the per-peak baseline, which 
                   "A window of 8 perfectly clustered cells shares 1.26x (21 % fewer gathered bytes) while every gathered "
                   "operand row would have to be applied to 8 accumulator rows under predication (8x the FMA issue for 1.26x "
                   "fewer loads); generation order gives 1.21x, so clustering buys almost nothing.  Reuse only becomes large "
-                  "(>2x) at W >= 32-64, where the window is simply dense in its columns -- the regime of the shared-memory "
-                  "panel kernel (spmm_panel.cu), which is bound by the same 128 B/clk L1/shared data pipe.  Hence the "
+                  "(>2x) at W >= 32-64, where the window is simply dense in its columns -- the regime where the operand is "
+                  "staged in shared memory, which is bound by the same 128 B/clk L1/shared data pipe.  Hence the "
                   "round-2 lever taken instead: fewer BYTES per gathered element (IEEE-half operand in the early block-"
-                  "Lanczos steps, spmm.cu::spmm_row_h).")
+                  "Lanczos steps, spmm.cu::spmm_row with T = __half).")
 print(json.dumps(out, indent=1))

@@ -67,7 +67,7 @@ def test_to_device_to_host_large(cuda):
 
 # ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("P", [32, 64, 128])
-def test_spmm_half_operand(cuda, P):
+def test_spmm_with_half_operand(cuda, P):
     """C = A @ half(B) with fp32 accumulation: equal to the float64 product with the SAME rounded operand to
     fp32 summation accuracy, for the CSR layout and the pair layout (transposed panels)."""
     X = tfidf_ref(generate_host(700, 900, 0.06, n_topics=6, seed=5)).astype(np.float32)
@@ -80,9 +80,9 @@ def test_spmm_half_operand(cuda, P):
     assert np.abs(Bh_ref - B.cpu().numpy()).max() < 2.0 ** -11 * np.abs(B.cpu().numpy()).max() * 1.01
     ref = X.astype(np.float64) @ Bh_ref
     for dyn in (False, True):
-        C = _device.spmm_h16(A, Bh, dynamic=dyn).cpu().numpy()
+        C = _device.spmm(A, Bh, dynamic=dyn).cpu().numpy()
         assert np.abs(C - ref).max() <= 2e-6 * np.abs(ref).max()
-    C2 = _device.spmm_h16(A, Bh, out=torch.ones((700, P), device=cuda), accumulate=True).cpu().numpy()
+    C2 = _device.spmm(A, Bh, out=torch.ones((700, P), device=cuda), accumulate=True).cpu().numpy()
     assert np.abs(C2 - 1.0 - ref).max() <= 3e-6 * max(1.0, np.abs(ref).max())
     # pair layout: (A^T) @ half(U)
     U = torch.randn((700, P), generator=g, device=cuda) / 25.0
