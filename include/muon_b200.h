@@ -137,6 +137,24 @@ int mub_spmm_csrp_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_row
 int mub_csrp_row_stats_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, double* sum,
                            double* sumsq, mub_stream_t stream);
 
+/* ---- CSR row-and-column selection: out = A[rows][:, kept columns], the kept columns renumbered.  Cuts a
+ * device-resident MOFA view into (view, group) blocks restricted to its use_var features, the work of the scipy
+ * fancy indexing X[rows][:, mask] on the host path (muon/_core/tools.py:172-176, 243-255).
+ * rows[n_rows_out]: int64 source row of every output row (repeats and any order allowed; NULL = every row, then
+ * n_rows_out == n_rows_src); the caller checks that every id is in [0, n_rows_src).  col_map[n_cols_src]: int32 new
+ * column of every source column, -1 = dropped (NULL = keep every column); a map that is increasing on the kept
+ * columns keeps sorted rows sorted.  indptr values are absolute offsets (they need not start at 0 and may exceed 2^31).
+ *   count : out_len[n_rows_out] (int64) = kept entries of every output row; an inclusive scan of it, behind a leading
+ *           0, is out_indptr.
+ *   fill  : writes out_indices / out_data at out_indptr (absolute offsets), entry order within a row preserved.  No
+ *           entry is written outside its output row's range, and a row with no kept entry is not read. */
+int mub_csr_select_count(const int64_t* indptr, const int32_t* indices, int64_t n_rows_src, int32_t n_cols_src,
+                         const int64_t* rows, int64_t n_rows_out, const int32_t* col_map, int64_t* out_len,
+                         mub_stream_t stream);
+int mub_csr_select_fill_f32(const int64_t* indptr, const int32_t* indices, const float* data, int32_t n_cols_src,
+                            const int64_t* rows, int64_t n_rows_out, const int32_t* col_map, const int64_t* out_indptr,
+                            int32_t* out_indices, float* out_data, mub_stream_t stream);
+
 /* ---- tall-skinny Gram (the k x k contraction that is allreduced across cell shards) ------
  * G[l x l] = Y^T Y for Y[n x ld] row-major, float64 result (partials are fp32 per CTA slab,
  * combined in fp64 in a fixed order: deterministic).  Replaces the dense Gram inside

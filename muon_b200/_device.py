@@ -472,6 +472,111 @@ def tfidf_csr(A: DeviceCSR, log_tf=True, log_idf=True, log_tfidf=False, scale_fa
     return res
 
 
+def row_range(rows, n: int):
+    """(lo, hi) if ``rows`` (None = all n rows, else a 1-D integer array) is the ascending range lo, lo+1, ..., hi-1,
+    else None.  An empty list is the empty range (0, 0)."""
+    if rows is None:
+        return 0, n
+    r = np.asarray(rows)
+    if r.size == 0:
+        return 0, 0
+    lo = int(r[0])
+    return (lo, lo + r.size) if np.array_equal(r, np.arange(lo, lo + r.size)) else None
+
+
+def select_is_view(rows, col_mask, n: int) -> bool:
+    """True when ``csr_select(A, rows, col_mask)`` of an n-row A returns a view of A's arrays (nothing copied): no
+    column mask and the rows an ascending range.  Otherwise the selected entries are gathered into new arrays."""
+    return col_mask is None and row_range(rows, n) is not None
+
+
+def attach_block_counts(A: DeviceCSR) -> DeviceCSR:
+    """Give A the per-(row chunk, column) and per-(512-row block, column) entry counts that TransposedPanels needs for
+    the deterministic tiled fill: the TF-IDF reduce pass run with flags = 0, its sums discarded.  A row that is not
+    sorted leaves A without counts (the panels then take the atomic-cursor fill), and so does
+    MUON_B200_TFIDF_TILED=0, which turns the tiled reduce pass off everywhere."""
+    n, d = A.shape
+    if not tiled_reduce_enabled() or not A.sorted_indices or n == 0 or d == 0 or A.data.dtype != torch.float32:
+        return A
+    dev = A.data.device
+    bounds = chunk_bounds(n)
+    counts = torch.zeros((N_CHUNKS, d), dtype=torch.int32, device=dev)
+    rb_counts = torch.empty((-(-n // tile_rows()), d), dtype=torch.int16, device=dev)
+    row_sum = torch.empty(n, dtype=torch.float32, device=dev)
+    col_sum = torch.zeros(d, dtype=torch.float32, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    call("mub_tfidf_reduce_tiled_f32", ptr(A.indptr), ptr(A.indices), ptr(A.data), n, d, ptr(row_sum), ptr(col_sum),
+         ptr(status), 0, ptr(counts), ptr(torch.tensor(bounds, dtype=torch.int64, device=dev)), N_CHUNKS, 0,
+         ptr(rb_counts), stream_ptr())
+    if int(status[0]) & 1:
+        A.sorted_indices = False
+        return A
+    aux = getattr(A, "_aux", None) or {}
+    aux.update({"col_counts": (bounds, counts), "rb_counts": rb_counts})
+    A._aux = aux
+    return A
+
+
+def csr_select(A: DeviceCSR, rows=None, col_mask=None) -> DeviceCSR:
+    """``A[rows][:, col_mask]`` on the device (csrc/select.cu), as a new DeviceCSR with float32 values.
+
+    ``rows``: source row of every output row (int array, any order, repeats allowed; None = all rows).  ``col_mask``:
+    boolean per column of A (None = keep all); the kept columns are renumbered in order, so sorted rows stay sorted.
+    An ascending row range without a column mask is a view: ``indices`` / ``data`` are narrowed, not copied, and only
+    ``indptr`` is rebased (8 B per row).  Anything else is counted, scanned and filled into new arrays (8 B per kept
+    entry).  ``select_is_view`` states the rule.  With ``rows=None`` the result keeps A's shard position (``row0``,
+    ``n_total``); any other row selection is a matrix of its own (row0 = 0, n_total = its height).  Every result
+    carries the entry counts of the deterministic transposition fill (``attach_block_counts``)."""
+    require_cuda()
+    assert A.data.dtype == torch.float32, "csr_select: float32 values only (convert fp64 first)"
+    n_src, d = A.shape
+    dev = A.data.device
+    st = stream_ptr()
+    col_map, d_out = None, d
+    if col_mask is not None:
+        mask = np.asarray(col_mask.cpu() if isinstance(col_mask, torch.Tensor) else col_mask, dtype=bool).reshape(-1)
+        if mask.shape[0] != d:
+            raise ValueError(f"csr_select: col_mask has {mask.shape[0]} entries, the matrix {d} columns")
+        cmap = np.full(d, -1, dtype=np.int32)
+        d_out = int(mask.sum())
+        cmap[mask] = np.arange(d_out, dtype=np.int32)
+        col_map = torch.from_numpy(cmap).to(dev)
+    r_host = None
+    if rows is not None:
+        r_host = np.asarray(rows.cpu() if isinstance(rows, torch.Tensor) else rows).reshape(-1)
+        if r_host.size and r_host.dtype.kind not in "iu":
+            raise TypeError(f"csr_select: rows must be integers, got {r_host.dtype}")
+        r_host = r_host.astype(np.int64, copy=False)
+        if r_host.size and (int(r_host.min()) < 0 or int(r_host.max()) >= n_src):
+            raise IndexError(f"csr_select: row ids must lie in [0, {n_src}), got [{int(r_host.min())}, {int(r_host.max())}]")
+    n_out = n_src if r_host is None else int(r_host.size)
+    # every row, in order: the same cells, so the same place in a cell-sharded matrix
+    shard = {"row0": A.row0, "n_total": A._n_total} if r_host is None else {"row0": 0, "n_total": n_out}
+    if select_is_view(r_host, col_mask, n_src):
+        lo, hi = row_range(r_host, n_src)
+        k0, k1 = (int(x) for x in A.indptr[[lo, hi]].tolist())
+        out = DeviceCSR(A.indptr[lo:hi + 1] - k0, A.indices[k0:k1], A.data[k0:k1], (n_out, d),
+                        sorted_indices=A.sorted_indices, **shard)
+        return attach_block_counts(out)
+    if n_out == 0:
+        return DeviceCSR(torch.zeros(1, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int32, device=dev),
+                         torch.empty(0, dtype=torch.float32, device=dev), (0, d_out), sorted_indices=A.sorted_indices,
+                         **shard)
+    rows_dev = None if r_host is None else torch.from_numpy(np.ascontiguousarray(r_host)).to(dev)
+    lens = torch.zeros(n_out + 1, dtype=torch.int64, device=dev)
+    call("mub_csr_select_count", ptr(A.indptr), ptr(A.indices), n_src, d, ptr(rows_dev), n_out, ptr(col_map),
+         ptr(lens) + 8, st)
+    indptr = torch.cumsum(lens, 0)
+    del lens
+    nnz = int(indptr[-1])
+    indices = torch.empty(nnz, dtype=torch.int32, device=dev)
+    data = torch.empty(nnz, dtype=torch.float32, device=dev)
+    call("mub_csr_select_fill_f32", ptr(A.indptr), ptr(A.indices), ptr(A.data), d, ptr(rows_dev), n_out, ptr(col_map),
+         ptr(indptr), ptr(indices), ptr(data), st)
+    out = DeviceCSR(indptr, indices, data, (n_out, d_out), sorted_indices=A.sorted_indices, **shard)
+    return attach_block_counts(out)
+
+
 def csr_transpose(A: DeviceCSR, row0: int = 0, row1: Optional[int] = None, k0: Optional[int] = None,
                   k1: Optional[int] = None, pairs: bool = False, col_count: Optional[torch.Tensor] = None,
                   rb_counts: Optional[torch.Tensor] = None, scratch: Optional[dict] = None):

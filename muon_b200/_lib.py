@@ -40,6 +40,8 @@ SIGNATURES = {
     "mub_csr_transpose_fill_pairs": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp],
     "mub_spmm_csrp_f32": [vp, vp, i64, i64, vp, i32, vp, i32, vp, vp],
     "mub_csrp_row_stats_f32": [vp, vp, i64, vp, vp, vp],
+    "mub_csr_select_count": [vp, vp, i64, i32, vp, i64, vp, vp, vp],
+    "mub_csr_select_fill_f32": [vp, vp, vp, i32, vp, i64, vp, vp, vp, vp, vp],
     "mub_mofa_update_w_f32": [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, vp],
     "mub_mofa_update_z_f32": [vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, vp],
     "mub_mofa_tau_f32": [vp, vp, vp, f64, vp, vp, vp, vp, f64, vp, i64, i32, i32, vp],

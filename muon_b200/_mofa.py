@@ -18,8 +18,16 @@ evaluated by fused low-rank kernels (csrc/mofa_lowrank.cu; ``MUON_B200_MOFA_PSEU
 path taken is recorded in ``uns["mofa"]["_b200"]["pseudo"]``), ``groups_label``, ``use_obs`` union /
 intersection (cells missing from whole views), ``use_var`` feature subsets, ``use_layer``, ``scale_views``,
 ``scale_groups``, ``center_groups``, ARD on weights / factors, spike-and-slab weights, convergence modes, ``copy``;
-the one-group case also cell-sharded over several GPUs.  Not supported (``NotImplementedError``, never a silent
-substitute): ``spikeslab_factors``, ``use_raw``, SVI, MEFISTO smoothing; ``outfile`` (HDF5) is ignored (h5py is not
+the one-group case also cell-sharded over several GPUs.  Views may be host matrices or device-resident ``DeviceCSR``
+(e.g. left in ``adata.X`` by ``tfidf``) in every combination of these options: a device view is cut into its (view,
+group) blocks and restricted to its ``use_var`` features on the device (csrc/select.cu), never downloaded.  A block
+that is an ascending run of the view's rows without a feature mask is a view of the view's arrays; any other block
+is gathered, which costs one extra copy of the view's kept entries (8 B per non-zero) in all.  Every device block
+carries the entry counts of the deterministic transposition fill, so such a fit is bit-reproducible.  What each
+block was made of is recorded in ``uns["mofa"]["_b200"]["blocks"]`` ({view: "slice" / "gather" / "host" per group;
+a device view with float64 values is first copied to float32 values, recorded as "convert+slice" / "convert+gather"}).
+Not supported (``NotImplementedError``, never a silent substitute): ``spikeslab_factors``, ``use_raw``, SVI, MEFISTO
+smoothing, groups / ``use_obs`` / ``scale_groups`` over several processes; ``outfile`` (HDF5) is ignored (h5py is not
 available); ``n_factors`` > 64.
 """
 from __future__ import annotations
@@ -599,17 +607,25 @@ def _to_device_view(X):
     return _device.DeviceCSR.from_scipy(Xs, dtype=np.float32)
 
 
-def _guess_likelihood(X) -> str:
+def _guess_likelihood(X, col_mask=None) -> str:
     """mofapy2's ``guess_likelihoods`` (reached from muon/_core/tools.py:272-280) on one view: bernoulli if every
     value is 0 or 1, poisson if every value is an integer, else gaussian.  Implicit zeros of a sparse matrix are
-    integers, so only the stored values need looking at (all of them, not a sample)."""
+    integers, so only the stored values need looking at (all of them, not a sample).  ``col_mask`` (DeviceCSR only):
+    look at the stored values of the kept columns only, as the host path does after subsetting; the value array is
+    masked chunk by chunk on the device, the matrix is not copied."""
     if isinstance(X, _device.DeviceCSR):
-        vals = X.data
-        if vals.numel() == 0:
-            return "bernoulli"
-        if not bool((vals == vals.round()).all()):
-            return "gaussian"
-        return "bernoulli" if bool(((vals == 0) | (vals == 1)).all()) else "poisson"
+        keep = None if col_mask is None else torch.from_numpy(np.array(col_mask, dtype=bool)).to(X.data.device)
+        integer = binary = True
+        step = 1 << 26                                      # bounds the temporaries
+        for k0 in range(0, X.nnz, step):
+            vals = X.data[k0:k0 + step]
+            if keep is not None:
+                vals = vals[keep[X.indices[k0:k0 + step]]]
+            integer = integer and bool((vals == vals.round()).all())
+            if not integer:
+                return "gaussian"
+            binary = binary and bool(((vals == 0) | (vals == 1)).all())
+        return "bernoulli" if binary else "poisson"
     vals = X.data if hasattr(X, "data") and not isinstance(X, np.ndarray) else np.asarray(X).ravel()
     vals = np.asarray(vals)
     vals = vals[~np.isnan(vals)] if vals.dtype.kind == "f" else vals
@@ -670,6 +686,48 @@ def _to_dense_device(X, dev) -> torch.Tensor:
         raise NotImplementedError("missing values (NaN) inside a non-gaussian view are not supported; drop the cells "
                                   "from the view and use use_obs='union'")
     return torch.from_numpy(np.ascontiguousarray(arr, dtype=np.float32)).to(dev)
+
+
+def _cell_layout(mdata, obs_all, common_obs, use_obs, groups_label):
+    """Cells of the general path in factor-matrix order: the selected cells ordered by group (tools.py:243-255).
+    Returns (cells, group id per cell, group names, (lo, hi) per group)."""
+    sel = obs_all if use_obs != "intersection" else obs_all[np.isin(obs_all, common_obs.astype(str))]
+    if groups_label is not None:                       # groups in order of first appearance, tools.py:215-219
+        glab_all = np.asarray(mdata.obs[groups_label]).astype(str)
+        glab = glab_all[np.isin(obs_all, sel)] if len(sel) != len(obs_all) else glab_all
+        group_names = list(dict.fromkeys(glab.tolist()))
+    else:
+        glab = np.array(["group1"] * len(sel))
+        group_names = ["group1"]
+    gid = np.array([group_names.index(x) for x in glab])
+    perm = np.argsort(gid, kind="stable")
+    gid = gid[perm]
+    bounds = np.searchsorted(gid, np.arange(len(group_names) + 1))
+    group_ranges = [(int(bounds[g]), int(bounds[g + 1])) for g in range(len(group_names))]
+    return sel[perm], gid, group_names, group_ranges
+
+
+def _view_rows(names, pos_of, group_ranges):
+    """Rows of one view per group, in factor-matrix order: [(view rows, their positions in Z)] per group, and the Z
+    positions of every selected row of the view."""
+    here = np.array([pos_of.get(c, -1) for c in names], dtype=np.int64)   # position of each of the view's rows in Z
+    keep = np.nonzero(here >= 0)[0]
+    order = keep[np.argsort(here[keep], kind="stable")]                     # view rows in Z order
+    zpos = here[order]
+    per_g = []
+    for lo, hi in group_ranges:
+        selg = (zpos >= lo) & (zpos < hi)
+        per_g.append((order[selg], zpos[selg]))
+    return per_g, zpos
+
+
+def _block_kind(X, rows, col_mask) -> str:
+    """How a (view, group) block of the device-resident view X is made by ``_device.csr_select(X, rows, col_mask)``
+    (rows None = all of them): "slice" (a view of the view's arrays, nothing copied) or "gather" (the block's kept
+    entries copied), by the rule csr_select itself applies.  A view with float64 values is first copied to float32
+    values (4 B per non-zero, indices shared), which the kind records as a "convert+" prefix."""
+    kind = "slice" if _device.select_is_view(rows, col_mask, X.shape[0]) else "gather"
+    return kind if X.data.dtype == torch.float32 else "convert+" + kind
 
 
 def mofa(
@@ -759,47 +817,64 @@ def mofa(
     if groups_label is not None and (not hasattr(mdata.obs, "columns") or groups_label not in mdata.obs.columns):
         raise KeyError(f"{groups_label} is not in observations names")     # reference prints and exits, tools.py:98-101
 
+    simple = (use_obs is None and groups_label is None and not scale_groups)
+    if not simple and _dist.is_distributed():
+        raise NotImplementedError("groups_label / use_obs need host matrices on a single process for now")
     _device.require_cuda()
     import scipy.sparse as sp
     dev = torch.device("cuda", torch.cuda.current_device())
     mods = list(mdata.mod.keys())
     M = len(mods)
     obs_all = np.asarray(mdata.obs_names).astype(str)
-    simple = (use_obs is None and groups_label is None and not scale_groups)
 
     # ---- features (tools.py:172-176) -----------------------------------------------------------------------
-    Xs, masks = [], []
+    # A device-resident view keeps all its columns here: its use_var mask (col_masks) is applied on the device, by the
+    # one selection that also cuts it into (view, group) blocks, so its kept entries are copied at most once.
+    Xs, masks, col_masks = [], [], []
     for m in mods:
         adata = mdata.mod[m]
         X = adata.layers[use_layer] if use_layer else adata.X
-        mask = None
+        mask = cmask = None
         if use_var and hasattr(adata.var, "columns") and use_var in adata.var.columns:
             mask = np.asarray(adata.var[use_var].astype(bool))
             if isinstance(X, _device.DeviceCSR):
-                raise NotImplementedError("use_var with a device-resident matrix is not supported yet")
-            X = (X.tocsr() if sp.issparse(X) else np.asarray(X))[:, mask]
+                cmask = None if mask.all() else mask
+            else:
+                X = (X.tocsr() if sp.issparse(X) else np.asarray(X))[:, mask]
         elif use_var:
             mask = np.ones(adata.n_vars, dtype=bool)
         Xs.append(X)
         masks.append(mask)
+        col_masks.append(cmask)
+    shapes = [(X.shape[0], X.shape[1] if cm is None else int(cm.sum())) for X, cm in zip(Xs, col_masks)]
 
     if lik is None:
         # The reference lets mofapy2 guess the likelihood per view (tools.py:272-280, mofapy2 guess_likelihoods):
         # all values in {0,1} -> bernoulli, all integers -> poisson, else gaussian.
-        lik = [_guess_likelihood(X) for X in Xs]
+        lik = [_guess_likelihood(X, cm) for X, cm in zip(Xs, col_masks)]
     mode = os.environ.get("MUON_B200_MOFA_PSEUDO", "auto")
     free = torch.cuda.mem_get_info(dev)[0]
     pseudo = {}
-    for m, X, l in zip(mods, Xs, lik):
+    for m, X, shape, l in zip(mods, Xs, shapes, lik):
         if l != "gaussian":
-            pseudo[m] = _pseudo_path(isinstance(X, _device.DeviceCSR) or sp.issparse(X), X.shape, free, mode)
+            pseudo[m] = _pseudo_path(isinstance(X, _device.DeviceCSR) or sp.issparse(X), shape, free, mode)
             if pseudo[m] == "dense":
-                _check_dense_fits(m, X.shape, l, dev)
+                _check_dense_fits(m, shape, l, dev)
 
     def pseudo_obs(m, X):                                 # observations of a poisson / bernoulli view (or block)
         return _to_dense_device(X, dev) if pseudo[m] == "dense" else _to_sparse_pseudo_view(X)
 
+    # what each (view, group) block is made of: "slice" of a device view (no copy), "gather" (its kept entries copied
+    # on the device), "host" (cut on the host and uploaded)
+    blocks_plan = {}
     if simple:
+        for i, (m, X, cm) in enumerate(zip(mods, Xs, col_masks)):
+            if isinstance(X, _device.DeviceCSR):
+                blocks_plan[m] = [_block_kind(X, None, cm)]
+                if cm is not None:
+                    Xs[i] = _device.csr_select(_to_device_view(X), col_mask=cm)
+            else:
+                blocks_plan[m] = ["host"]
         views = [_to_device_view(X) if l == "gaussian" else pseudo_obs(m, X) for m, X, l in zip(mods, Xs, lik)]
         sparse_views = [v for v in views if isinstance(v, _device.DeviceCSR)]
         n_local = views[0].shape[0]
@@ -819,52 +894,47 @@ def mofa(
         group_names = ["group1"]
         variance = {m: res["variance"][i].cpu().numpy() for i, m in enumerate(mods)}
     else:
-        # ---- general path: groups of cells and/or cells missing from whole views (host matrices) ---------------
-        if any(isinstance(X, _device.DeviceCSR) for X in Xs) or _dist.is_distributed():
-            raise NotImplementedError("groups_label / use_obs need host matrices on a single process for now")
-        sel = obs_all if use_obs != "intersection" else obs_all[np.isin(obs_all, common_obs.astype(str))]
-        if groups_label is not None:                       # groups in order of first appearance, tools.py:215-219
-            glab_all = np.asarray(mdata.obs[groups_label]).astype(str)
-            glab = glab_all[np.isin(obs_all, sel)] if len(sel) != len(obs_all) else glab_all
-            group_names = list(dict.fromkeys(glab.tolist()))
-        else:
-            glab = np.array(["group1"] * len(sel))
-            group_names = ["group1"]
-        gid = np.array([group_names.index(x) for x in glab])
-        perm = np.argsort(gid, kind="stable")               # cells ordered by group (tools.py:243-255)
-        cells = sel[perm]
-        gid = gid[perm]
+        # ---- general path: groups of cells and/or cells missing from whole views ----------------------------------
+        # A device-resident view is cut into its (view, group) blocks on the device (csrc/select.cu); a host matrix is
+        # cut on the host and every block uploaded.
+        cells, gid, group_names, group_ranges = _cell_layout(mdata, obs_all, common_obs, use_obs, groups_label)
         N = len(cells)
         G = len(group_names)
-        bounds = np.searchsorted(gid, np.arange(G + 1))
-        group_ranges = [(int(bounds[g]), int(bounds[g + 1])) for g in range(G)]
         pos_of = {c: i for i, c in enumerate(cells)}
         bits = np.zeros(N, dtype=np.int64)
         blocks, dims = [], []
         for mi, m in enumerate(mods):
             names = np.asarray(mdata.mod[m].obs_names).astype(str)
-            X = Xs[mi]
-            X = X.tocsr() if sp.issparse(X) else sp.csr_matrix(np.asarray(X))
-            here = np.array([pos_of.get(c, -1) for c in names])     # position of each of the view's rows in Z
-            keep = np.nonzero(here >= 0)[0]
-            order = keep[np.argsort(here[keep], kind="stable")]      # view rows in Z order
-            zpos = here[order]
+            X = src = Xs[mi]
+            on_device = isinstance(X, _device.DeviceCSR)
+            if on_device:
+                X = _to_device_view(X)
+            else:
+                X = X.tocsr() if sp.issparse(X) else sp.csr_matrix(np.asarray(X))
+            per_rows, zpos = _view_rows(names, pos_of, group_ranges)
             bits[zpos] |= (1 << mi)
-            per_g = []
+            per_g, kinds = [], []
             for g, (lo, hi) in enumerate(group_ranges):
-                selg = (zpos >= lo) & (zpos < hi)
-                rows_z = zpos[selg]
-                Xg = X[order[selg]].astype(np.float32)
-                if lik[mi] == "gaussian":
-                    A = _device.DeviceCSR.from_scipy(sp.csr_matrix(Xg), dtype=np.float32)
+                rows_v, rows_z = per_rows[g]
+                if on_device:
+                    kinds.append(_block_kind(src, rows_v, col_masks[mi]))
+                    Ag = _device.csr_select(X, rows_v, col_masks[mi])
+                    A = Ag if lik[mi] == "gaussian" else pseudo_obs(m, Ag)
                 else:
-                    A = pseudo_obs(m, Xg)
+                    kinds.append("host")
+                    Xg = X[rows_v].astype(np.float32)
+                    if lik[mi] == "gaussian":
+                        A = _device.DeviceCSR.from_scipy(sp.csr_matrix(Xg), dtype=np.float32)
+                    else:
+                        A = pseudo_obs(m, Xg)
                 if len(rows_z) == hi - lo and np.array_equal(rows_z, np.arange(lo, hi)):
                     per_g.append((A, (lo, hi)))
                 else:
                     per_g.append((A, torch.from_numpy(rows_z.astype(np.int64)).to(dev)))
             blocks.append(per_g)
-            dims.append(X.shape[1])
+            blocks_plan[m] = kinds
+            dims.append(shapes[mi][1])
+            del X
         cls = torch.from_numpy(((gid << M) | bits).astype(np.int32)).to(dev)
         rs = np.random.RandomState(seed)
         Z0 = torch.from_numpy(rs.normal(size=(N, n_factors)))
@@ -906,7 +976,7 @@ def mofa(
         "variance": variance,
     }
     data.uns["mofa"]["_b200"] = {"iterations": res["iterations"], "converged": res["converged"], "elbo": res["elbo"],
-                                 "pseudo": pseudo}
+                                 "pseudo": pseudo, "blocks": blocks_plan}
     if copy:
         return data
     if not quiet:
