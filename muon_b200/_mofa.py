@@ -19,8 +19,11 @@ path taken is recorded in ``uns["mofa"]["_b200"]["pseudo"]``), ``groups_label``,
 intersection (cells missing from whole views), ``use_var`` feature subsets, ``use_layer``, ``scale_views``,
 ``scale_groups``, ``center_groups``, ARD on weights / factors, spike-and-slab weights, convergence modes, ``copy``;
 the one-group case also cell-sharded over several GPUs.  Views may be host matrices or device-resident ``DeviceCSR``
-(e.g. left in ``adata.X`` by ``tfidf``) in every combination of these options: a device view is cut into its (view,
-group) blocks and restricted to its ``use_var`` features on the device (csrc/select.cu), never downloaded.  A block
+(e.g. left in ``adata.X`` by ``tfidf``) in every combination of these options.  Every call is marshalled the same
+way: ``_layout`` orders the cells by group and finds the rows of every view in each group (with no ``groups_label``,
+``use_obs`` or ``scale_groups``, row i of every view is cell i and no names are matched), ``_block`` cuts each (view,
+group) block, and one ``MofaDevice`` is trained.  A device view is cut into its blocks and restricted to its
+``use_var`` features on the device (csrc/select.cu), never downloaded.  A block
 that is an ascending run of the view's rows without a feature mask is a view of the view's arrays; any other block
 is gathered, which costs one extra copy of the view's kept entries (8 B per non-zero) in all.  Every device block
 carries the entry counts of the deterministic transposition fill, so such a fit is bit-reproducible.  What each
@@ -50,26 +53,38 @@ TOLERANCE = {"fast": 5e-4, "medium": 5e-5, "slow": 5e-6}
 f64 = torch.float64
 
 
-class _Block:
-    """One (view, group) block: the cells of group g observed in view m, as a compact CSR with its
-    transpose panels, plus where those cells sit in the local factor matrix."""
+class _Rows:
+    """What every (view, group) block shares: the cells of group g observed in view m, and where they sit in the local
+    factor matrix (``rows``: LongTensor into the local Z, or None = Z[lo:hi])."""
 
-    def __init__(self, A: _device.DeviceCSR, rows, lo: int, hi: int, ld: int):
-        self.A, self.At = A, A.transpose_panels(ld)
-        self.rows, self.lo, self.hi = rows, lo, hi      # rows: LongTensor into local Z, or None = Z[lo:hi]
-        self.n_local = A.shape[0]
+    P_at_end = False                                     # Yhat^T E[Z] formed only for the variance explained
+
+    def __init__(self, rows, lo: int, hi: int, n_local: int):
+        self.rows, self.lo, self.hi, self.n_local = rows, lo, hi, n_local
 
     def take(self, Z):                                   # rows of Z belonging to this block (contiguous n x ld)
         return Z[self.lo:self.hi] if self.rows is None else Z.index_select(0, self.rows)
 
+    def add_av(self, Q, tw):
+        """Q[rows of the block] += Y_b (tau * W): accumulated in place on a row range, else formed and scattered"""
+        if self.rows is None:
+            self._av(tw, Q[self.lo:self.hi])
+        else:
+            Q.index_add_(0, self.rows, self._av(tw, None))
+
+
+class _Block(_Rows):
+    """One (view, group) block of a gaussian view: a compact CSR with its transpose panels."""
+
+    def __init__(self, A: _device.DeviceCSR, rows, lo: int, hi: int, ld: int):
+        super().__init__(rows, lo, hi, A.shape[0])
+        self.A, self.At = A, A.transpose_panels(ld)
+
     def aty(self, Zb):                                   # Y_b^T Z_b  (D x ld): transposed sparse pass
         return self.At.spmm(Zb.contiguous(), dynamic=True)
 
-    def add_av(self, Q, tw):                             # Q[rows of the block] += Y_b (tau * W)
-        if self.rows is None:
-            _device.spmm(self.A, tw, out=Q[self.lo:self.hi], accumulate=True, dynamic=False)
-        else:
-            Q.index_add_(0, self.rows, _device.spmm(self.A, tw, dynamic=False))
+    def _av(self, tw, out):                              # Y_b tw, accumulated onto out if given
+        return _device.spmm(self.A, tw, out=out, accumulate=out is not None, dynamic=False)
 
     def moments(self, D, dev):
         """per-feature sum and sum of squares over the block's cells (fp64), from the transposed panels"""
@@ -82,28 +97,38 @@ class _Block:
         return s1, s2
 
 
-class _DenseBlock:
+class _DenseBlock(_Rows):
     """One (view, group) block of a NON-gaussian view: the observations as a dense row-major fp32 matrix and the
     Seeger pseudo-data that stand in for them (dense by construction: zeta = E[Z] E[W]^T is).  The contractions
     are GEMMs (cuBLAS via torch); the elementwise passes are csrc/mofa_pseudo.cu."""
 
-    def __init__(self, obs: torch.Tensor, rows, lo: int, hi: int):
+    def __init__(self, obs: torch.Tensor, rows, lo: int, hi: int, kind: int):
         assert obs.dtype == torch.float32 and obs.is_contiguous() and obs.dim() == 2
+        super().__init__(rows, lo, hi, obs.shape[0])
         self.obs, self.Y = obs, torch.zeros_like(obs)
-        self.rows, self.lo, self.hi = rows, lo, hi
-        self.n_local = obs.shape[0]
+        self.kind = kind
 
-    def take(self, Z):
-        return Z[self.lo:self.hi] if self.rows is None else Z.index_select(0, self.rows)
+    def col_max(self, D, dev):
+        return self.obs.max(0).values
+
+    def pseudo(self, Zb, W, kappa, K):
+        """form the pseudo-data at zeta = Zb W^T; return (Yhat^T Zb, sum_n Yhat^2 per feature)"""
+        torch.matmul(Zb[:, :K], W[:, :K].contiguous().T, out=self.Y)
+        call("mub_mofa_pseudo_f32", ptr(self.Y), ptr(self.obs), ptr(kappa), self.n_local, self.obs.shape[1], self.kind,
+             stream_ptr())
+        return self.aty(Zb), (self.Y * self.Y).sum(0, dtype=f64)
 
     def aty(self, Zb):
         return self.Y.T @ Zb
 
-    def add_av(self, Q, tw):
-        if self.rows is None:
-            Q[self.lo:self.hi].addmm_(self.Y, tw)
-        else:
-            Q.index_add_(0, self.rows, self.Y @ tw)
+    def _av(self, tw, out):
+        return self.Y @ tw if out is None else out.addmm_(self.Y, tw)
+
+    def loglik(self, Zb, W, K, acc):
+        """acc += sum over the block's cells and all features of ln p(y | zeta) at zeta = Zb W^T"""
+        zeta = Zb[:, :K].contiguous() @ W[:, :K].contiguous().T
+        call("mub_mofa_loglik_f32", ptr(zeta), ptr(self.obs), self.n_local, self.obs.shape[1], self.kind, ptr(acc),
+             stream_ptr())
 
 
 def _padded(X, K):
@@ -113,22 +138,21 @@ def _padded(X, K):
     return out
 
 
-class _SparsePseudoBlock:
+class _SparsePseudoBlock(_Rows):
     """One (view, group) block of a NON-gaussian view kept sparse: the observations as a CSR with its transpose panels.
     The pseudo-data are never stored.  They are g(zeta) everywhere plus a correction s at the stored entries
     (csrc/mofa_lowrank.cu), with zeta = Z_zeta W_zeta^T at the factors the current pseudo-data were formed at, so a
     copy of those factors is kept.  Contractions: a low-rank sweep for the g part plus a gathering pass over the
-    non-zeros."""
+    non-zeros.  Yhat^T E[Z] costs a low-rank sweep and only the variance explained reads it (the next pseudo-data
+    overwrite it), so it is formed once, after the last iteration."""
+
+    P_at_end = True
 
     def __init__(self, A: _device.DeviceCSR, rows, lo: int, hi: int, ld: int, kind: int):
+        super().__init__(rows, lo, hi, A.shape[0])
         self.A, self.At = A, A.transpose_panels(ld)
-        self.rows, self.lo, self.hi = rows, lo, hi
-        self.n_local = A.shape[0]
         self.ld, self.kind = ld, kind
         self.Zz = self.Wz = self.kappa = None            # no pseudo-data formed yet: Yhat = 0
-
-    def take(self, Z):
-        return Z[self.lo:self.hi] if self.rows is None else Z.index_select(0, self.rows)
 
     def col_max(self, D, dev):
         """max over the block's cells of every feature, implicit zeros counting as 0"""
@@ -162,9 +186,10 @@ class _SparsePseudoBlock:
                  ptr(self.kappa), ptr(C) + row * r0, self.ld, self.kind, ptr(P), ptr(ssq), st)
         return P, ssq
 
-    def add_av(self, Q, tw):                             # Q[rows of the block] += Yhat (tau * W)
+    def _av(self, tw, out):                              # Yhat tw, accumulated onto out if given
         n, D, st = self.n_local, self.At.shape[0], stream_ptr()
-        out = Q[self.lo:self.hi] if self.rows is None else torch.zeros((n, self.ld), dtype=torch.float32, device=Q.device)
+        if out is None:
+            out = torch.zeros((n, self.ld), dtype=torch.float32, device=tw.device)
         call("mub_mofa_lowrank_rows_f32", ptr(self.Zz), n, ptr(self.Wz), D, ptr(self.kappa), ptr(tw), self.ld, self.kind,
              ptr(out), 1, None, st)
         if self.kind == 2:                               # bernoulli: s = y / kappa is linear in y
@@ -172,8 +197,7 @@ class _SparsePseudoBlock:
         else:
             call("mub_mofa_nnz_rows_f32", ptr(self.A.indptr), ptr(self.A.indices), ptr(self.A.data), n, ptr(self.Zz),
                  ptr(self.Wz), ptr(self.kappa), ptr(tw), self.ld, self.kind, ptr(out), None, st)
-        if self.rows is not None:
-            Q.index_add_(0, self.rows, out)
+        return out
 
     def loglik(self, Zb, W, K, acc):
         """acc += sum over the block's cells and all features of ln p(y | zeta) at zeta = Zb W^T"""
@@ -203,10 +227,8 @@ class _View:
                 continue
             if self.kind == 0:
                 s1[g], s2[g] = b.moments(D, dev)
-            elif isinstance(b, _SparsePseudoBlock):
-                mx = torch.maximum(mx, b.col_max(D, dev))
             else:
-                mx = torch.maximum(mx, b.obs.max(0).values)
+                mx = torch.maximum(mx, b.col_max(D, dev))
         if self.kind != 0:
             # non-gaussian view: no centring, no scaling, precision fixed at Seeger's bound (oracle/mofa_ref.py)
             _dist.all_reduce_sum_(cnt)
@@ -336,12 +358,13 @@ class MofaDevice:
             for g in range(self.G):
                 A, rows = blocks[m][g]
                 r, lo, hi = (None, rows[0], rows[1]) if isinstance(rows, tuple) else (rows, 0, 0)
+                kind = 1 if self.liks[m] == "poisson" else 2
                 if self.liks[m] == "gaussian":
                     bl.append(_Block(A, r, lo, hi, ld))
                 elif isinstance(A, _device.DeviceCSR):    # non-gaussian view kept sparse
-                    bl.append(_SparsePseudoBlock(A, r, lo, hi, ld, 1 if self.liks[m] == "poisson" else 2))
+                    bl.append(_SparsePseudoBlock(A, r, lo, hi, ld, kind))
                 else:                                     # A: dense fp32 observations (n_b x D) on the device
-                    bl.append(_DenseBlock(A, r, lo, hi))
+                    bl.append(_DenseBlock(A, r, lo, hi, kind))
             self.views.append(_View(bl, dims[m], K, ld, center, scale_views, scale_groups, dev, self.liks[m]))
         self.Z = torch.zeros((self.n_local, ld), dtype=torch.float32, device=dev)
         self.Z[:, :K] = Z0.to(dev, torch.float32)
@@ -359,9 +382,7 @@ class MofaDevice:
         K = self.K
         dK = torch.arange(K, device=self.dev)
         for m, v in enumerate(self.views):
-            # Yhat^T E[Z] of a sparse non-gaussian view is read only by variance_explained() (the next _pseudo
-            # overwrites it), so it is formed there, once, instead of a low-rank sweep per iteration
-            v.P_stale = any(isinstance(b, _SparsePseudoBlock) for b in v.blocks)
+            v.P_stale = any(b.P_at_end for b in v.blocks)          # formed by variance_explained() instead
             for g, b in enumerate(v.blocks):
                 if b.n_local > 0:
                     Zb = b.take(self.Z)
@@ -458,37 +479,21 @@ class MofaDevice:
     def _pseudo(self, v):
         """Seeger pseudo-data of a non-gaussian view around zeta = E[Z] E[W]^T (csrc/mofa_pseudo.cu), then the
         statistics of the view that depend on them: P = Yhat^T E[Z] and sum Yhat^2 per feature."""
-        K, st = self.K, stream_ptr()
-        Wk = v.W[:, :K].contiguous()
         for g, b in enumerate(v.blocks):
             if b.n_local == 0:
                 v.P[g].zero_()
                 v.ssq[g].zero_()
-                continue
-            Zb = b.take(self.Z).contiguous()
-            if isinstance(b, _SparsePseudoBlock):
-                v.P[g], v.ssq[g] = b.pseudo(Zb, v.W, v.kappa32, K)
-                continue
-            torch.matmul(Zb[:, :K], Wk.T, out=b.Y)
-            call("mub_mofa_pseudo_f32", ptr(b.Y), ptr(b.obs), ptr(v.kappa32), b.n_local, v.D, v.kind, st)
-            v.P[g] = b.aty(Zb)
-            v.ssq[g] = (b.Y * b.Y).sum(0, dtype=f64)
+            else:
+                v.P[g], v.ssq[g] = b.pseudo(b.take(self.Z).contiguous(), v.W, v.kappa32, self.K)
         _dist.all_reduce_sum_(v.P)
         _dist.all_reduce_sum_(v.ssq)
 
     def _loglik(self, v):
         """sum over the observed entries of ln p(y | zeta) at zeta = E[Z] E[W]^T (the ELBO term of a non-gaussian view)"""
-        K, st = self.K, stream_ptr()
         acc = torch.zeros(1, dtype=f64, device=self.dev)
-        Wk = v.W[:, :K].contiguous()
         for b in v.blocks:
-            if b.n_local == 0:
-                continue
-            if isinstance(b, _SparsePseudoBlock):
-                b.loglik(b.take(self.Z), v.W, K, acc)
-                continue
-            zeta = b.take(self.Z)[:, :K].contiguous() @ Wk.T
-            call("mub_mofa_loglik_f32", ptr(zeta), ptr(b.obs), b.n_local, v.D, v.kind, ptr(acc), st)
+            if b.n_local > 0:
+                b.loglik(b.take(self.Z), v.W, self.K, acc)
         return float(_dist.all_reduce_sum_(acc)[0])
 
     def _elbo(self):
@@ -585,8 +590,9 @@ def _train(model, n_iterations, convergence_mode, check_convergence, sort_factor
 def run_mofa_device(views, n_factors, n_iterations, n_total, Z0, center=True, scale_views=False, ard_weights=True,
                     ard_factors=True, spikeslab_weights=True, convergence_mode="fast", check_convergence=True,
                     sort_factors=True, verbose=False, likelihoods=None):
-    """One group, every cell observed in every view (the benchmark case).  ``views``: per modality a DeviceCSR
-    (gaussian) or a dense fp32 device tensor (poisson / bernoulli, see ``likelihoods``) of this rank's cells.
+    """One group, every cell observed in every view: the model ``mofa()`` builds for such a call, on views already on
+    the device (the benchmark case).  ``views``: per modality a DeviceCSR, or the dense fp32 observations of a poisson
+    / bernoulli view (see ``likelihoods``) on the dense pseudo-data path, of this rank's cells.
     Returns dict(Z, W (list), variance (list of K-vectors), elbo, iterations, converged)."""
     n_local = views[0].shape[0]
     blocks = [[(A, (0, n_local))] for A in views]
@@ -689,7 +695,7 @@ def _to_dense_device(X, dev) -> torch.Tensor:
 
 
 def _cell_layout(mdata, obs_all, common_obs, use_obs, groups_label):
-    """Cells of the general path in factor-matrix order: the selected cells ordered by group (tools.py:243-255).
+    """Cells of a name-matching layout in factor-matrix order: the selected cells ordered by group (tools.py:243-255).
     Returns (cells, group id per cell, group names, (lo, hi) per group)."""
     sel = obs_all if use_obs != "intersection" else obs_all[np.isin(obs_all, common_obs.astype(str))]
     if groups_label is not None:                       # groups in order of first appearance, tools.py:215-219
@@ -721,6 +727,39 @@ def _view_rows(names, pos_of, group_ranges):
     return per_g, zpos
 
 
+def _layout(mdata, Xs, obs_all, common_obs, use_obs, groups_label, identity: bool):
+    """The cells of the factor matrix and the rows of every view in each group.  Returns (rows, group names, (lo, hi)
+    and global cell count per group, (row0, n_total), cells): ``rows[m][g]`` = (view m's rows in group g in
+    factor-matrix order, None = all of them in order; their factor-matrix rows, (lo, hi) or an int64 array); the
+    local cells' initial factors are rows row0 .. of a draw for n_total cells; ``cells`` = (name, class id = group
+    << M | views observed in) per factor-matrix row, None = every cell in every view, in order.
+
+    The identity layout (``identity``: no ``groups_label``, ``use_obs`` or ``scale_groups``) takes row i of every
+    view as cell i, matching no names, where the first DeviceCSR view places it (a cell shard, masked or not, keeps
+    its place; host matrices alone are rows 0 .. of all processes' cells).  Any other layout matches the views' rows
+    by name to the cells of ``_cell_layout``, row0 = 0 and n_total = N."""
+    if identity:
+        n = Xs[0].shape[0]
+        dv = next((X for X in Xs if isinstance(X, _device.DeviceCSR)), None)
+        if dv is not None:
+            row0, n_total = dv.row0, dv.n_total
+        else:
+            cnt = torch.tensor([n], dtype=torch.int64, device="cuda") if _dist.is_distributed() else None
+            row0, n_total = 0, n if cnt is None else int(_dist.all_reduce_sum_(cnt)[0])
+        return [[(None, (0, n))] for _ in Xs], ["group1"], [(0, n)], [n_total], (row0, n_total), None
+    cells, gid, group_names, group_ranges = _cell_layout(mdata, obs_all, common_obs, use_obs, groups_label)
+    pos_of = {c: i for i, c in enumerate(cells)}
+    bits = np.zeros(len(cells), dtype=np.int64)
+    rows = []
+    for m, ad in enumerate(mdata.mod.values()):
+        per_g, zpos = _view_rows(np.asarray(ad.obs_names).astype(str), pos_of, group_ranges)
+        bits[zpos] |= 1 << m
+        rows.append([(rv, (lo, hi) if np.array_equal(rz, np.arange(lo, hi)) else rz)
+                     for (rv, rz), (lo, hi) in zip(per_g, group_ranges)])
+    cls = ((gid << len(rows)) | bits).astype(np.int32)
+    return rows, group_names, group_ranges, [hi - lo for lo, hi in group_ranges], (0, len(cells)), (cells, cls)
+
+
 def _block_kind(X, rows, col_mask) -> str:
     """How a (view, group) block of the device-resident view X is made by ``_device.csr_select(X, rows, col_mask)``
     (rows None = all of them): "slice" (a view of the view's arrays, nothing copied) or "gather" (the block's kept
@@ -728,6 +767,23 @@ def _block_kind(X, rows, col_mask) -> str:
     values (4 B per non-zero, indices shared), which the kind records as a "convert+" prefix."""
     kind = "slice" if _device.select_is_view(rows, col_mask, X.shape[0]) else "gather"
     return kind if X.data.dtype == torch.float32 else "convert+" + kind
+
+
+def _block(X, rows, col_mask, pseudo, dev):
+    """Rows ``rows`` (None = all, in order) and features ``col_mask`` of view X (float32 values if on the device; a
+    host matrix comes restricted to its features) as the fit holds them: a DeviceCSR, or dense observations on the
+    dense pseudo-data path (``pseudo``: None for a gaussian view, else "dense" / "sparse").  A device view is cut on
+    the device, or used as it is when nothing is cut (its cached transposed panels and entry counts are kept); a
+    host matrix is cut on the host, or uploaded as it is."""
+    import scipy.sparse as sp
+    if isinstance(X, _device.DeviceCSR):
+        if rows is not None or col_mask is not None:
+            X = _device.csr_select(X, rows, col_mask)
+    elif rows is not None:
+        X = (X.tocsr()[rows] if sp.issparse(X) else sp.csr_matrix(np.asarray(X)[rows])).astype(np.float32)
+    if pseudo == "dense":
+        return _to_dense_device(X, dev)
+    return _to_device_view(X) if pseudo is None else _to_sparse_pseudo_view(X)
 
 
 def mofa(
@@ -817,15 +873,13 @@ def mofa(
     if groups_label is not None and (not hasattr(mdata.obs, "columns") or groups_label not in mdata.obs.columns):
         raise KeyError(f"{groups_label} is not in observations names")     # reference prints and exits, tools.py:98-101
 
-    simple = (use_obs is None and groups_label is None and not scale_groups)
-    if not simple and _dist.is_distributed():
+    identity = (use_obs is None and groups_label is None and not scale_groups)     # see _layout
+    if not identity and _dist.is_distributed():
         raise NotImplementedError("groups_label / use_obs need host matrices on a single process for now")
     _device.require_cuda()
     import scipy.sparse as sp
     dev = torch.device("cuda", torch.cuda.current_device())
     mods = list(mdata.mod.keys())
-    M = len(mods)
-    obs_all = np.asarray(mdata.obs_names).astype(str)
 
     # ---- features (tools.py:172-176) -----------------------------------------------------------------------
     # A device-resident view keeps all its columns here: its use_var mask (col_masks) is applied on the device, by the
@@ -861,95 +915,38 @@ def mofa(
             if pseudo[m] == "dense":
                 _check_dense_fits(m, shape, l, dev)
 
-    def pseudo_obs(m, X):                                 # observations of a poisson / bernoulli view (or block)
-        return _to_dense_device(X, dev) if pseudo[m] == "dense" else _to_sparse_pseudo_view(X)
-
-    # what each (view, group) block is made of: "slice" of a device view (no copy), "gather" (its kept entries copied
-    # on the device), "host" (cut on the host and uploaded)
-    blocks_plan = {}
-    if simple:
-        for i, (m, X, cm) in enumerate(zip(mods, Xs, col_masks)):
-            if isinstance(X, _device.DeviceCSR):
-                blocks_plan[m] = [_block_kind(X, None, cm)]
-                if cm is not None:
-                    Xs[i] = _device.csr_select(_to_device_view(X), col_mask=cm)
-            else:
-                blocks_plan[m] = ["host"]
-        views = [_to_device_view(X) if l == "gaussian" else pseudo_obs(m, X) for m, X, l in zip(mods, Xs, lik)]
-        sparse_views = [v for v in views if isinstance(v, _device.DeviceCSR)]
-        n_local = views[0].shape[0]
-        if sparse_views:
-            n_total, row0 = sparse_views[0].n_total, sparse_views[0].row0
-        elif _dist.is_distributed():
-            raise NotImplementedError("cell-sharded mofa() needs at least one gaussian (DeviceCSR) view to carry the shard offsets")
-        else:
-            n_total, row0 = n_local, 0
-        rs = np.random.RandomState(seed)
-        Z0 = torch.from_numpy(rs.normal(size=(n_total, n_factors))[row0:row0 + n_local])
-        res = run_mofa_device(views, n_factors, n_iterations, n_total, Z0, center=center_groups,
-                              scale_views=scale_views, ard_weights=ard_weights, ard_factors=ard_factors,
-                              spikeslab_weights=spikeslab_weights, convergence_mode=convergence_mode,
-                              verbose=verbose and not quiet, likelihoods=lik)
-        Z_full = res["Z"].cpu().numpy()
-        group_names = ["group1"]
-        variance = {m: res["variance"][i].cpu().numpy() for i, m in enumerate(mods)}
-    else:
-        # ---- general path: groups of cells and/or cells missing from whole views ----------------------------------
-        # A device-resident view is cut into its (view, group) blocks on the device (csrc/select.cu); a host matrix is
-        # cut on the host and every block uploaded.
-        cells, gid, group_names, group_ranges = _cell_layout(mdata, obs_all, common_obs, use_obs, groups_label)
-        N = len(cells)
-        G = len(group_names)
-        pos_of = {c: i for i, c in enumerate(cells)}
-        bits = np.zeros(N, dtype=np.int64)
-        blocks, dims = [], []
-        for mi, m in enumerate(mods):
-            names = np.asarray(mdata.mod[m].obs_names).astype(str)
-            X = src = Xs[mi]
-            on_device = isinstance(X, _device.DeviceCSR)
-            if on_device:
-                X = _to_device_view(X)
-            else:
-                X = X.tocsr() if sp.issparse(X) else sp.csr_matrix(np.asarray(X))
-            per_rows, zpos = _view_rows(names, pos_of, group_ranges)
-            bits[zpos] |= (1 << mi)
-            per_g, kinds = [], []
-            for g, (lo, hi) in enumerate(group_ranges):
-                rows_v, rows_z = per_rows[g]
-                if on_device:
-                    kinds.append(_block_kind(src, rows_v, col_masks[mi]))
-                    Ag = _device.csr_select(X, rows_v, col_masks[mi])
-                    A = Ag if lik[mi] == "gaussian" else pseudo_obs(m, Ag)
-                else:
-                    kinds.append("host")
-                    Xg = X[rows_v].astype(np.float32)
-                    if lik[mi] == "gaussian":
-                        A = _device.DeviceCSR.from_scipy(sp.csr_matrix(Xg), dtype=np.float32)
-                    else:
-                        A = pseudo_obs(m, Xg)
-                if len(rows_z) == hi - lo and np.array_equal(rows_z, np.arange(lo, hi)):
-                    per_g.append((A, (lo, hi)))
-                else:
-                    per_g.append((A, torch.from_numpy(rows_z.astype(np.int64)).to(dev)))
-            blocks.append(per_g)
-            blocks_plan[m] = kinds
-            dims.append(shapes[mi][1])
-            del X
-        cls = torch.from_numpy(((gid << M) | bits).astype(np.int32)).to(dev)
-        rs = np.random.RandomState(seed)
-        Z0 = torch.from_numpy(rs.normal(size=(N, n_factors)))
-        model = MofaDevice(blocks, dims, group_ranges, [hi - lo for lo, hi in group_ranges], cls, n_factors, Z0,
-                           center_groups, scale_views, scale_groups, ard_weights, ard_factors, spikeslab_weights, lik)
-        res = _train(model, n_iterations, convergence_mode, True, True, verbose and not quiet)
-        Zp = res["Z"].cpu().numpy()
+    # ---- (view, group) blocks: a device view is cut on the device (csrc/select.cu), a host matrix on the host -------
+    obs_all = np.asarray(mdata.obs_names).astype(str)
+    rows, group_names, group_ranges, n_groups, (row0, n_total), cells = _layout(
+        mdata, Xs, obs_all, common_obs, use_obs, groups_label, identity)
+    blocks, blocks_plan = [], {}
+    for m, src, cm, view_rows in zip(mods, Xs, col_masks, rows):
+        X = _to_device_view(src) if isinstance(src, _device.DeviceCSR) else src    # float64 values: one float32 copy
+        blocks.append([(_block(X, r, cm, pseudo.get(m), dev),
+                        z if isinstance(z, tuple) else torch.from_numpy(z).to(dev)) for r, z in view_rows])
+        blocks_plan[m] = [_block_kind(src, r, cm) if isinstance(src, _device.DeviceCSR) else "host"
+                          for r, _ in view_rows]
+        del X
+    if _dist.is_distributed() and not any(isinstance(A, _device.DeviceCSR) for per_g in blocks for A, _ in per_g):
+        raise NotImplementedError("cell-sharded mofa() needs at least one gaussian (DeviceCSR) view to carry the shard "
+                                  "offsets")
+    n = group_ranges[-1][1]
+    Z0 = torch.from_numpy(np.random.RandomState(seed).normal(size=(n_total, n_factors))[row0:row0 + n])
+    model = MofaDevice(blocks, [s[1] for s in shapes], group_ranges, n_groups,
+                       None if cells is None else torch.from_numpy(cells[1]).to(dev), n_factors, Z0, center_groups,
+                       scale_views, scale_groups, ard_weights, ard_factors, spikeslab_weights, lik)
+    res = _train(model, n_iterations, convergence_mode, True, True, verbose and not quiet)
+    Zp = res["Z"].cpu().numpy()
+    Z_full = Zp if cells is None else np.full((len(obs_all), n_factors), np.nan)     # tools.py:617-622
+    if cells is not None:
         where = {c: i for i, c in enumerate(obs_all)}
-        Z_full = np.full((len(obs_all), n_factors), np.nan)          # tools.py:617-622
-        Z_full[[where[c] for c in cells]] = Zp
-        if G > 1:                                                    # tools.py:690-697
-            variance = {m: {group_names[g]: res["variance"][i][g].cpu().numpy() for g in range(G)}
-                        for i, m in enumerate(mods)}
-        else:
-            variance = {m: res["variance"][i][0].cpu().numpy() for i, m in enumerate(mods)}
+        Z_full[[where[c] for c in cells[0]]] = Zp
+    G = len(group_names)
+    if G > 1:                                                    # tools.py:690-697
+        variance = {m: {group_names[g]: res["variance"][i][g].cpu().numpy() for g in range(G)}
+                    for i, m in enumerate(mods)}
+    else:
+        variance = {m: res["variance"][i][0].cpu().numpy() for i, m in enumerate(mods)}
 
     if copy:
         data = data.copy()

@@ -237,6 +237,29 @@ def test_union_and_device_views_match_dense_path(cuda, monkeypatch):
     np.testing.assert_allclose(auto.uns["mofa"]["_b200"]["elbo"], dense.uns["mofa"]["_b200"]["elbo"], rtol=1e-5)
 
 
+def test_one_group_mofa_fits_the_model_run_mofa_device_fits(cuda, monkeypatch):
+    """one-group mofa() on a gaussian and a bernoulli device view carrying entry counts, and run_mofa_device (what
+    bench.py times) with the same likelihoods, the initial factors mofa() draws, its convergence check and its factor
+    order: bit-identical fits"""
+    from muon_b200._mofa import run_mofa_device
+    from muon_b200._synth import generate_device
+    monkeypatch.setenv("MUON_B200_MOFA_PSEUDO", "sparse")
+    N, D, K, T, seed = 3000, 2000, 6, 15, 4
+    Xg = _device.attach_block_counts(_device.tfidf_csr(generate_device(N, D, 0.02, seed=5)))
+    Xb = _device.attach_block_counts(Xg.with_data(torch.ones_like(Xg.data)))
+    assert all("rb_counts" in X._aux for X in (Xg, Xb))
+    md = SimpleMuData({"cont": SimpleAnnData(Xg), "binary": SimpleAnnData(Xb)})
+    mu.tl.mofa(md, use_var=None, likelihoods=["gaussian", "bernoulli"], n_factors=K, n_iterations=T, seed=seed)
+    assert md.uns["mofa"]["_b200"]["pseudo"] == {"binary": "sparse"}
+    assert md.uns["mofa"]["_b200"]["blocks"] == {"cont": ["slice"], "binary": ["slice"]}
+    Z0 = np.random.RandomState(seed).normal(size=(Xg.n_total, K))[Xg.row0:Xg.row0 + N]
+    res = run_mofa_device([Xg, Xb], K, T, Xg.n_total, torch.from_numpy(Z0), likelihoods=["gaussian", "bernoulli"],
+                          check_convergence=True, sort_factors=True)
+    assert md.uns["mofa"]["_b200"]["elbo"] == res["elbo"]
+    assert np.array_equal(md.obsm["X_mofa"], res["Z"].cpu().numpy().astype(np.float64))
+    assert np.array_equal(md.varm["LFs"], np.concatenate([W.cpu().numpy() for W in res["W"]]).astype(np.float64))
+
+
 def test_views_too_large_for_dense_pseudo_data(cuda, monkeypatch):
     """150k x 120k poisson and bernoulli views at 1 %: dense pseudo-data would need 216 GB, the sparse path runs"""
     from muon_b200._synth import generate_device

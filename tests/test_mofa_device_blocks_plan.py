@@ -103,6 +103,49 @@ def test_empty_block_is_a_slice():
     assert plan["a"] == [("slice", [0, 1, 2]), ("slice", [])]
 
 
+def _shard(ad, row0=0, n_total=None):
+    """a device view of ad's shape that describes a cell shard (no entries; host tensors)"""
+    n, d = ad.shape
+    return _device.DeviceCSR(torch.zeros(n + 1, dtype=torch.int64), torch.empty(0, dtype=torch.int32),
+                             torch.empty(0, dtype=torch.float32), (n, d), row0, n_total)
+
+
+def test_identity_layout_takes_the_shard_of_the_first_device_view():
+    """one group, no use_obs: every view's rows are None (all of them, in order, no names matched), and the initial
+    factors' window and the group's cell count are the first DeviceCSR view's row0 / n_total"""
+    md = _md(6)
+    a, b = md.mod["a"], md.mod["b"]
+    obs_all = np.asarray(md.obs_names).astype(str)
+    host = sp.random(6, 4, density=0.5, format="csr")
+    for Xs, window in (([_shard(a, 200, 1000), _shard(b)], (200, 1000)),
+                       ([host, _shard(b, 40, 90)], (40, 90)),
+                       ([host, host], (0, 6))):
+        rows, names, ranges, totals, win, cells = _mofa._layout(md, Xs, obs_all, None, None, None, identity=True)
+        assert rows == [[(None, (0, 6))], [(None, (0, 6))]]
+        assert names == ["group1"] and ranges == [(0, 6)] and cells is None
+        assert win == window and totals == [window[1]]
+    # any other layout: the window is the N selected cells, whatever shard a view describes
+    names6 = [f"c{i}" for i in range(6)]
+    md2 = _md(6, obs_a=names6[:4], obs_b=names6[2:])
+    md2.obs["grp"] = np.array(["x", "y"] * 3)
+    obs_all = np.asarray(md2.obs_names).astype(str)
+    Xs = [_shard(md2.mod["a"], 200, 1000), _shard(md2.mod["b"])]
+    common = np.intersect1d(names6[:4], names6[2:])
+    for use_obs, n in (("union", 6), ("intersection", 2)):
+        rows, _, ranges, totals, win, (cells, cls) = _mofa._layout(md2, Xs, obs_all, common, use_obs, "grp",
+                                                                   identity=False)
+        assert win == (0, n) and sum(totals) == n and ranges[-1][1] == n
+        # every factor-matrix row (cells ordered by group), its group and the views it is observed in
+        want = [0, 2, 4, 1, 3, 5] if use_obs == "union" else [2, 3]
+        assert cells.tolist() == [f"c{p}" for p in want]
+        assert cls.tolist() == [((p % 2) << 2) | (p < 4) | ((p >= 2) << 1) for p in want]
+    # a block whose cells are one run of the factor matrix is a row range, any other one a list of rows
+    rows, *_ = _mofa._layout(md2, Xs, obs_all, common, "intersection", "grp", identity=False)
+    assert [z for _, z in rows[0]] == [(0, 1), (1, 2)]
+    rows, *_ = _mofa._layout(md2, Xs, obs_all, common, "union", "grp", identity=False)
+    assert [z.tolist() for _, z in rows[0]] == [[0, 1], [3, 4]]
+
+
 def test_distributed_general_path_is_refused(monkeypatch):
     md = _md(6)
     md.obs["grp"] = np.array(["x", "y"] * 3)
