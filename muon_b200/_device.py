@@ -414,38 +414,67 @@ def chunk_bounds(n: int, align: Optional[int] = None) -> list:
     return b
 
 
-def tiled_reduce_enabled() -> bool:
-    return os.environ.get("MUON_B200_TFIDF_TILED", "1") != "0"
+class _EntryCounts:
+    """The entry counts of an n x d matrix that TransposedPanels reads from ``A._aux``: ``col_counts`` =
+    (chunk_bounds(n), int32 [N_CHUNKS][d] per (row chunk, column)) and ``rb_counts`` = uint16 [ceil(n / 512)][d] per
+    (512-row block, column), held as int16.  The tiled TF-IDF reduce pass leaves them as a side product."""
+
+    def __init__(self, n: int, d: int, device):
+        self.bounds = chunk_bounds(n)
+        self.counts = torch.zeros((N_CHUNKS, d), dtype=torch.int32, device=device)
+        self._bounds_dev = torch.tensor(self.bounds, dtype=torch.int64, device=device)
+        self.rb_counts = torch.empty((-(-n // tile_rows()), d), dtype=torch.int16, device=device)
+
+    def reduce(self, A: DeviceCSR, row_sum, col_sum, status, flags: int, r0: int = 0, r1: Optional[int] = None,
+               stream=None):
+        """The tiled reduce pass (shared-memory tiles, ~30x fewer global atomics than mub_tfidf_reduce_f32) over rows
+        [r0, r1) of A, float32 values, r0 a multiple of the tile height: their sums into row_sum[r0:r1], their column
+        sums added to col_sum, their entry counts into these buffers, the canonical-form verdict ORed into status.
+        Bit0 of the verdict (a row not sorted) means none of the sums or counts are valid."""
+        n, d = A.shape
+        r1 = n if r1 is None else r1
+        call("mub_tfidf_reduce_tiled_f32", ptr(A.indptr) + 8 * r0, ptr(A.indices), ptr(A.data), r1 - r0, d,
+             ptr(row_sum) + 4 * r0, ptr(col_sum), ptr(status), flags, ptr(self.counts), ptr(self._bounds_dev), N_CHUNKS,
+             r0, ptr(self.rb_counts), stream_ptr() if stream is None else stream)
+
+    def record(self, A: DeviceCSR):
+        """Attach the counts to A: its transposed panels then skip the counting pass and take the tiled fill."""
+        aux = getattr(A, "_aux", None) or {}
+        aux.update({"col_counts": (self.bounds, self.counts), "rb_counts": self.rb_counts})
+        A._aux = aux
 
 
-def tfidf_csr(A: DeviceCSR, log_tf=True, log_idf=True, log_tfidf=False, scale_factor=1e4,
-              inplace_values=False, check_canonical=False, binarize=False) -> Optional[DeviceCSR]:
-    """K1: two fused passes (reduce, apply).  Column sums are allreduced across cell shards
-    (muon/_atac/preproc.py:92-119; multi-GPU plan SURVEY section 8e)."""
-    require_cuda()
-    n, d = A.shape
-    sfx = "f32" if A.data.dtype == torch.float32 else "f64"
+def _tfidf_flags(log_tf, log_idf, log_tfidf, scale_factor, binarize=False):
+    """The TF-IDF kernels' flag word and the scale factor they apply (1.0 when there is none)."""
     flags = (TFIDF_LOG_TF if log_tf else 0) | (TFIDF_LOG_IDF if log_idf else 0) | (TFIDF_LOG_TFIDF if log_tfidf else 0)
     if scale_factor is None or scale_factor == 0 or scale_factor == 1:
         flags |= TFIDF_NO_SCALE
         scale_factor = 1.0
     if binarize:
         flags |= TFIDF_BINARIZE
+    return flags, scale_factor
+
+
+def tfidf_csr(A: DeviceCSR, log_tf=True, log_idf=True, log_tfidf=False, scale_factor=1e4,
+              inplace_values=False, check_canonical=False, binarize=False) -> Optional[DeviceCSR]:
+    """K1: two fused passes (reduce, apply).  Column sums are allreduced across cell shards
+    (muon/_atac/preproc.py:92-119; multi-GPU plan SURVEY section 8e).  float32 values with sorted rows take the tiled
+    reduce pass, and the result carries the entry counts of its transposition; anything else takes the order-agnostic
+    kernel and carries none."""
+    require_cuda()
+    n, d = A.shape
+    sfx = "f32" if A.data.dtype == torch.float32 else "f64"
+    flags, scale_factor = _tfidf_flags(log_tf, log_idf, log_tfidf, scale_factor, binarize)
     dev, dt = A.data.device, A.data.dtype
     row_sum = torch.empty(n, dtype=dt, device=dev)
     col_sum = torch.zeros(d, dtype=dt, device=dev)
     st = stream_ptr()
     status = torch.zeros(1, dtype=torch.int32, device=dev) if check_canonical else None
     counts = None
-    if sfx == "f32" and A.sorted_indices and tiled_reduce_enabled() and n > 0:
-        # shared-memory tiled pass: column sums + the transposition's entry counts, ~30x fewer global atomics
+    if sfx == "f32" and A.sorted_indices and n > 0:
         st_t = torch.zeros(1, dtype=torch.int32, device=dev)
-        bounds = chunk_bounds(n)
-        counts = torch.zeros((N_CHUNKS, d), dtype=torch.int32, device=dev)
-        cb = torch.tensor(bounds, dtype=torch.int64, device=dev)
-        rb_counts = torch.empty((-(-n // tile_rows()), d), dtype=torch.int16, device=dev)      # uint16 entries per (512-row block, column)
-        call("mub_tfidf_reduce_tiled_f32", ptr(A.indptr), ptr(A.indices), ptr(A.data), n, d, ptr(row_sum), ptr(col_sum),
-             ptr(st_t), flags, ptr(counts), ptr(cb), N_CHUNKS, 0, ptr(rb_counts), st)
+        counts = _EntryCounts(n, d, dev)
+        counts.reduce(A, row_sum, col_sum, st_t, flags, stream=st)
         bad = int(st_t[0])
         if check_canonical and bad != 0:
             return None  # caller canonicalises (duplicates / explicit zeros / unsorted rows) and retries
@@ -467,8 +496,7 @@ def tfidf_csr(A: DeviceCSR, log_tf=True, log_idf=True, log_tfidf=False, scale_fa
     res = A.with_data(out)
     res._aux = {"row_sum": row_sum, "col_sum": col_sum, "idf": idf}
     if counts is not None:
-        res._aux["col_counts"] = (bounds, counts)
-        res._aux["rb_counts"] = rb_counts
+        counts.record(res)
     return res
 
 
@@ -492,28 +520,21 @@ def select_is_view(rows, col_mask, n: int) -> bool:
 
 def attach_block_counts(A: DeviceCSR) -> DeviceCSR:
     """Give A the per-(row chunk, column) and per-(512-row block, column) entry counts that TransposedPanels needs for
-    the deterministic tiled fill: the TF-IDF reduce pass run with flags = 0, its sums discarded.  A row that is not
-    sorted leaves A without counts (the panels then take the atomic-cursor fill), and so does
-    MUON_B200_TFIDF_TILED=0, which turns the tiled reduce pass off everywhere."""
+    the deterministic tiled fill: the TF-IDF reduce pass run with flags = 0, its sums discarded.  A matrix whose rows
+    are not sorted, or whose values are not float32, is left without counts (its panels then take the atomic-cursor
+    fill)."""
     n, d = A.shape
-    if not tiled_reduce_enabled() or not A.sorted_indices or n == 0 or d == 0 or A.data.dtype != torch.float32:
+    if not A.sorted_indices or n == 0 or d == 0 or A.data.dtype != torch.float32:
         return A
     dev = A.data.device
-    bounds = chunk_bounds(n)
-    counts = torch.zeros((N_CHUNKS, d), dtype=torch.int32, device=dev)
-    rb_counts = torch.empty((-(-n // tile_rows()), d), dtype=torch.int16, device=dev)
-    row_sum = torch.empty(n, dtype=torch.float32, device=dev)
-    col_sum = torch.zeros(d, dtype=torch.float32, device=dev)
+    counts = _EntryCounts(n, d, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
-    call("mub_tfidf_reduce_tiled_f32", ptr(A.indptr), ptr(A.indices), ptr(A.data), n, d, ptr(row_sum), ptr(col_sum),
-         ptr(status), 0, ptr(counts), ptr(torch.tensor(bounds, dtype=torch.int64, device=dev)), N_CHUNKS, 0,
-         ptr(rb_counts), stream_ptr())
+    counts.reduce(A, torch.empty(n, dtype=torch.float32, device=dev), torch.zeros(d, dtype=torch.float32, device=dev),
+                  status, 0)
     if int(status[0]) & 1:
         A.sorted_indices = False
-        return A
-    aux = getattr(A, "_aux", None) or {}
-    aux.update({"col_counts": (bounds, counts), "rb_counts": rb_counts})
-    A._aux = aux
+    else:
+        counts.record(A)
     return A
 
 
@@ -577,55 +598,32 @@ def csr_select(A: DeviceCSR, rows=None, col_mask=None) -> DeviceCSR:
     return attach_block_counts(out)
 
 
-def csr_transpose(A: DeviceCSR, row0: int = 0, row1: Optional[int] = None, k0: Optional[int] = None,
-                  k1: Optional[int] = None, pairs: bool = False, col_count: Optional[torch.Tensor] = None,
-                  rb_counts: Optional[torch.Tensor] = None, scratch: Optional[dict] = None):
-    """Build the CSR of (A[row0:row1])^T on the device (count -> scan -> atomic-cursor fill).
-    Row indices stored in the result are local to the panel (0 .. row1-row0).  ``k0``/``k1`` are the
-    non-zero offsets of the row range if the caller already knows them (avoids a host sync)."""
+def _transposed_indptr(A: DeviceCSR, k0: int, k1: int, col_count: Optional[torch.Tensor]) -> torch.Tensor:
+    """Row offsets of the transpose of the rows of A that hold the non-zeros [k0, k1): scanned from ``col_count`` (their
+    entries per column) when it is known, else from a counting pass."""
+    d = A.shape[1]
+    t_count = torch.zeros(d + 1, dtype=torch.int64, device=A.data.device)
+    if col_count is not None:
+        t_count[1:] = col_count
+    else:
+        call("mub_csr_transpose_count", ptr(A.indices) + 4 * k0, k1 - k0, d, ptr(t_count), stream_ptr())
+    return torch.cumsum(t_count, 0)
+
+
+def csr_transpose(A: DeviceCSR) -> DeviceCSR:
+    """The CSR of A^T on the device (count -> scan -> atomic-cursor fill).  The order of the entries inside a transposed
+    row follows the fill's slot claims."""
     require_cuda()
     assert A.data.dtype == torch.float32, "transpose: float32 values only"
     n, d = A.shape
-    row1 = n if row1 is None else row1
     dev = A.data.device
-    st = stream_ptr()
-    if k0 is None or k1 is None:
-        if row0 == 0 and row1 == n:
-            k0, k1 = 0, A.nnz
-        else:
-            k0, k1 = int(A.indptr[row0]), int(A.indptr[row1])
-    nnz = k1 - k0
-    t_count = torch.zeros(d + 1, dtype=torch.int64, device=dev)
-    if col_count is not None:      # entries per column of this row range, known from the TF-IDF reduce pass
-        t_count[1:] = col_count
-    else:
-        call("mub_csr_transpose_count", ptr(A.indices) + 4 * k0, nnz, d, ptr(t_count), st)
-    t_indptr = torch.cumsum(t_count, 0)
+    t_indptr = _transposed_indptr(A, 0, A.nnz, None)
     cursor = torch.empty(max(d, 1), dtype=torch.int64, device=dev)
-    if pairs and rb_counts is not None and col_count is not None and row0 % tile_rows() == 0:
-        # atomic-free fill: write offsets of every 512-row block from the scanned per-block counts (transpose.cu)
-        t_pairs = torch.empty((nnz, 2), dtype=torch.int32, device=dev)
-        nb = -(-(row1 - row0) // tile_rows())
-        if scratch.get("base") is None or scratch["base"].numel() < nb * d:
-            scratch["base"] = torch.empty(nb * d, dtype=torch.int32, device=dev)
-        if scratch.get("status") is None:
-            scratch["status"] = torch.zeros(1, dtype=torch.int32, device=dev)
-        call("mub_csr_transpose_fill_tiled", ptr(A.indptr) + 8 * row0, ptr(A.indices), ptr(A.data), row1 - row0, d,
-             ptr(rb_counts) + 2 * (row0 // tile_rows()) * d, ptr(t_indptr), ptr(scratch["base"]), ptr(t_pairs),
-             ptr(scratch["status"]), st)
-        return DevicePairs(t_indptr, t_pairs, (d, row1 - row0))
-    if pairs:
-        t_pairs = torch.empty((nnz, 2), dtype=torch.int32, device=dev)
-        call("mub_csr_transpose_fill_pairs", ptr(A.indptr) + 8 * row0, ptr(A.indices), ptr(A.data), row1 - row0, d, 0,
-             ptr(t_indptr), ptr(cursor), ptr(t_pairs), st)
-        return DevicePairs(t_indptr, t_pairs, (d, row1 - row0))
-    t_indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-    t_data = torch.empty(nnz, dtype=torch.float32, device=dev)
-    # indptr values are absolute offsets into indices/data, so only the indptr pointer is shifted;
-    # slots claimed from `cursor` are panel-local, so the outputs are not
-    call("mub_csr_transpose_fill", ptr(A.indptr) + 8 * row0, ptr(A.indices), ptr(A.data), row1 - row0, d, 0,
-         ptr(t_indptr), ptr(cursor), ptr(t_indices), ptr(t_data), st)
-    return DeviceCSR(t_indptr, t_indices, t_data, (d, row1 - row0), n_total=d, sorted_indices=False)
+    t_indices = torch.empty(A.nnz, dtype=torch.int32, device=dev)
+    t_data = torch.empty(A.nnz, dtype=torch.float32, device=dev)
+    call("mub_csr_transpose_fill", ptr(A.indptr), ptr(A.indices), ptr(A.data), n, d, 0, ptr(t_indptr), ptr(cursor),
+         ptr(t_indices), ptr(t_data), stream_ptr())
+    return DeviceCSR(t_indptr, t_indices, t_data, (d, n), n_total=d, sorted_indices=False)
 
 
 class TransposedPanels:
@@ -637,7 +635,7 @@ class TransposedPanels:
     L2_BUDGET = int(os.environ.get("MUON_B200_L2_BUDGET_MB", "16")) << 20
 
     def __init__(self, A: DeviceCSR, pad: int = 64):
-        n = A.shape[0]
+        n, d = A.shape
         rows = max(1, self.L2_BUDGET // (4 * pad))
         n_panels = max(1, -(-n // rows))
         counts, rb = None, None
@@ -653,28 +651,46 @@ class TransposedPanels:
                 cc = aux["col_counts"][1]
                 counts = [cc[i * per:(i + 1) * per].sum(0, dtype=torch.int64) for i in range(n_panels)]
                 # the tiled fill lists every transposed row in ascending cell order, so A^T Y sums in the same
-                # order on every run (the atomic-cursor fill's order follows slot claims); MUON_B200_FILL_TILED=0
-                # selects the atomic-cursor fill
-                if os.environ.get("MUON_B200_FILL_TILED", "1") == "1":
-                    rb = aux.get("rb_counts")
+                # order on every run (the atomic-cursor fill's order follows slot claims)
+                rb = aux.get("rb_counts")
         else:
             bounds = [round(i * n / n_panels) for i in range(n_panels + 1)]
         self.counts_reused = counts is not None
         self.tiled_fill = False
-        self.shape = (A.shape[1], n)
+        self.shape = (d, n)
         # non-zero offsets of the panel boundaries: one small D2H up front, no host syncs afterwards
         ks = A.indptr[torch.tensor(bounds, device=A.indptr.device)].tolist()
-        scratch = {}
-        build = lambda rbc: [(bounds[i], bounds[i + 1], csr_transpose(A, bounds[i], bounds[i + 1], ks[i], ks[i + 1], pairs=True,  # noqa: E731
-                                                                      col_count=counts[i] if counts else None, rb_counts=rbc,
-                                                                      scratch=scratch))
-                             for i in range(n_panels) if bounds[i + 1] > bounds[i]]
-        self.panels = build(rb)
+        spans = [(bounds[i], bounds[i + 1], ks[i], ks[i + 1], counts[i] if counts else None)
+                 for i in range(n_panels) if bounds[i + 1] > bounds[i]]
         if rb is not None:
-            if int(scratch["status"][0]) == 0:
-                self.tiled_fill = True
-            else:          # counts and pattern disagree (the matrix was modified after tfidf): atomic-cursor fill
-                self.panels = build(None)
+            # the scanned write offsets of the largest panel's 512-row blocks, reused by every panel
+            nb = max((-(-(r1 - r0) // tile_rows()) for r0, r1, *_ in spans), default=0)
+            tiled = (rb, torch.empty(nb * d, dtype=torch.int32, device=A.data.device),
+                     torch.zeros(1, dtype=torch.int32, device=A.data.device))
+            self.panels = [self._panel(A, *s, tiled=tiled) for s in spans]
+            self.tiled_fill = int(tiled[2][0]) == 0
+        if not self.tiled_fill:    # no per-block counts, or they disagree with the pattern (A modified after tfidf)
+            self.panels = [self._panel(A, *s) for s in spans]
+
+    @staticmethod
+    def _panel(A: DeviceCSR, r0: int, r1: int, k0: int, k1: int, col_count: Optional[torch.Tensor], tiled=None):
+        """(r0, r1, (A[r0:r1])^T) in the pairs layout, row indices local to the panel; k0/k1: the non-zero offsets of
+        rows r0 and r1.  ``tiled`` = (per-block counts, write-offset buffer, status word) selects the tiled fill, which
+        sets bit0 of the status word if the pattern disagrees with the counts; None the atomic-cursor fill."""
+        d = A.shape[1]
+        dev, st = A.data.device, stream_ptr()
+        t_indptr = _transposed_indptr(A, k0, k1, col_count)
+        t_pairs = torch.empty((k1 - k0, 2), dtype=torch.int32, device=dev)
+        # indptr values are absolute offsets into indices/data, so only the indptr pointer is shifted
+        if tiled is not None:
+            rb, base, status = tiled
+            call("mub_csr_transpose_fill_tiled", ptr(A.indptr) + 8 * r0, ptr(A.indices), ptr(A.data), r1 - r0, d,
+                 ptr(rb) + 2 * (r0 // tile_rows()) * d, ptr(t_indptr), ptr(base), ptr(t_pairs), ptr(status), st)
+        else:
+            cursor = torch.empty(max(d, 1), dtype=torch.int64, device=dev)
+            call("mub_csr_transpose_fill_pairs", ptr(A.indptr) + 8 * r0, ptr(A.indices), ptr(A.data), r1 - r0, d, 0,
+                 ptr(t_indptr), ptr(cursor), ptr(t_pairs), st)
+        return r0, r1, DevicePairs(t_indptr, t_pairs, (d, r1 - r0))
 
     def spmm(self, Y: torch.Tensor, dynamic=True, half: bool = False) -> torch.Tensor:
         """A^T Y accumulated panel by panel.  ``half``: round Y to IEEE half first (see ``spmm``)."""
@@ -784,7 +800,7 @@ def gram(Y: torch.Tensor, l: Optional[int] = None, weights: Optional[torch.Tenso
 _BLOCK_NNZ = int(os.environ.get("MUON_B200_BLOCK_NNZ", str(192 << 20)))
 
 
-def _row_blocks(indptr_host: np.ndarray, block_nnz: int, align: int = 1):
+def _row_blocks(indptr_host: np.ndarray, block_nnz: int, align: int):
     """Cut rows into consecutive blocks of about ``block_nnz`` stored entries -> list of (r0, r1, k0, k1); cuts are
     multiples of ``align`` rows."""
     n = indptr_host.shape[0] - 1
@@ -808,29 +824,23 @@ def tfidf_from_host(X, log_tf=True, log_idf=True, log_tfidf=False, scale_factor=
     assert X.data.dtype == np.float32
     n, d = X.shape
     dev = torch.device("cuda", torch.cuda.current_device())
-    flags = (TFIDF_LOG_TF if log_tf else 0) | (TFIDF_LOG_IDF if log_idf else 0) | (TFIDF_LOG_TFIDF if log_tfidf else 0)
-    if scale_factor is None or scale_factor == 0 or scale_factor == 1:
-        flags |= TFIDF_NO_SCALE
-        scale_factor = 1.0
+    flags, scale_factor = _tfidf_flags(log_tf, log_idf, log_tfidf, scale_factor)
     indptr_h = np.ascontiguousarray(X.indptr)
     indices_h = np.ascontiguousarray(X.indices)
     data_h = np.ascontiguousarray(X.data)
     nnz = int(indptr_h[-1]) if indptr_h.shape[0] else 0
-    tiled = tiled_reduce_enabled()
-    blocks = _row_blocks(indptr_h, _BLOCK_NNZ, tile_rows() if tiled else 1)
+    blocks = _row_blocks(indptr_h, _BLOCK_NNZ, tile_rows())
     st = stager()
     main = torch.cuda.current_stream()
     side = torch.cuda.Stream()
     indptr = to_device(indptr_h, dev, np.int64)
     indices = torch.empty(nnz, dtype=torch.int32, device=dev)
     data = torch.empty(nnz, dtype=torch.float32, device=dev)
+    res = DeviceCSR(indptr, indices, data, (n, d))
     row_sum = torch.empty(n, dtype=torch.float32, device=dev)
     col_sum = torch.zeros(d, dtype=torch.float32, device=dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
-    bounds = chunk_bounds(n) if tiled else None
-    counts = torch.zeros((N_CHUNKS, d), dtype=torch.int32, device=dev) if tiled else None
-    cb = torch.tensor(bounds, dtype=torch.int64, device=dev) if tiled else None
-    rb_counts = torch.empty((-(-n // tile_rows()), d), dtype=torch.int16, device=dev) if tiled else None
+    counts = _EntryCounts(n, d, dev)
     side.wait_stream(main)                      # allocations above are ordered on the main stream
     narrow = indices_h.dtype == np.int64
     assert narrow or indices_h.dtype == np.int32, indices_h.dtype
@@ -848,23 +858,15 @@ def tfidf_from_host(X, log_tf=True, log_idf=True, log_tfidf=False, scale_factor=
             as_u8 = False
             st.h2d(data_h[k0:k1], data[k0:k1], stream=side)
         main.wait_event(side.record_event())
-        if tiled:      # host matrices must be canonical anyway (checked here): sorted rows, so the tiled pass applies
-            call("mub_tfidf_reduce_tiled_f32", ptr(indptr) + 8 * r0, ptr(indices), ptr(data), r1 - r0, d, ptr(row_sum) + 4 * r0,
-                 ptr(col_sum), ptr(status), flags, ptr(counts), ptr(cb), N_CHUNKS, r0, ptr(rb_counts), main.cuda_stream)
-        else:
-            call("mub_tfidf_reduce_f32", ptr(indptr) + 8 * r0, ptr(indices), ptr(data), r1 - r0, d, ptr(row_sum) + 4 * r0,
-                 ptr(col_sum), ptr(status), flags, main.cuda_stream)
+        # host matrices must be canonical anyway (checked here): sorted rows, so the tiled pass applies
+        counts.reduce(res, row_sum, col_sum, status, flags, r0, r1, main.cuda_stream)
     for t in (indices, data):
         t.record_stream(side)
     if int(status[0]) != 0:                     # duplicates / explicit zeros / unsorted rows (also syncs the upload)
         return None
     _dist.all_reduce_sum_(col_sum)
     idf = torch.empty(d, dtype=torch.float32, device=dev)
-    n_total = n
-    if _dist.is_distributed():
-        t = torch.tensor([n], dtype=torch.int64, device=dev)
-        n_total = int(_dist.all_reduce_sum_(t)[0])
-    call("mub_tfidf_idf_f32", ptr(col_sum), d, float(n_total), flags, ptr(idf), main.cuda_stream)
+    call("mub_tfidf_idf_f32", ptr(col_sum), d, float(res.n_total), flags, ptr(idf), main.cuda_stream)
     with _timed("alloc_out_s"):
         out_h = _ARENA.empty(nnz, np.float32)
 
@@ -881,11 +883,8 @@ def tfidf_from_host(X, log_tf=True, log_idf=True, log_tfidf=False, scale_factor=
     ranges = [(k0, k1) for (_, _, k0, k1) in blocks]
     fp_idx = device_fingerprints(indices, ranges)
     fp_out = device_fingerprints(data, ranges)
-    res = DeviceCSR(indptr, indices, data, (n, d), n_total=n_total)
     res._aux = {"row_sum": row_sum, "col_sum": col_sum, "idf": idf}
-    if tiled:
-        res._aux["col_counts"] = (bounds, counts)
-        res._aux["rb_counts"] = rb_counts
+    counts.record(res)
     fps = {"blocks": [(k0, k1) for (_, _, k0, k1) in blocks], "indices": fp_idx, "data": fp_out,
            "indptr": host_pool().fingerprint(indptr_h.astype(np.int64, copy=False).view(np.uint32)) if n else 0}
     return res, out_h, fps

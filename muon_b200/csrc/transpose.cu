@@ -36,6 +36,21 @@ __global__ void copy_i64_kernel(const int64_t* __restrict__ src, int64_t* __rest
     if (i < n) dst[i] = src[i];
 }
 
+// PAIRS: (row, value) is written as ONE 8-byte pair (int2, in t_indices; t_data unused) instead of into two arrays:
+// one scattered store per non-zero instead of two (the fill is bound by the rate of scattered L2 operations, not by
+// bytes).
+template <bool PAIRS>
+__device__ __forceinline__ void store_entry(int32_t* __restrict__ t_indices, float* __restrict__ t_data,
+                                            unsigned long long slot, int32_t r, float v) {
+    if constexpr (PAIRS) {
+        reinterpret_cast<int2*>(t_indices)[slot] = make_int2(r, __float_as_int(v));
+    } else {
+        t_indices[slot] = r;
+        t_data[slot] = v;
+    }
+}
+
+template <bool PAIRS>
 __global__ void __launch_bounds__(256)
 transpose_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
                       const float* __restrict__ data, int64_t n_rows, int64_t row_offset,
@@ -55,52 +70,37 @@ transpose_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
             const float v2 = ld_stream(data + k + 64), v3 = ld_stream(data + k + 96);
             const unsigned long long s0 = atomicAdd(cursor + c0, 1ull), s1 = atomicAdd(cursor + c1, 1ull);
             const unsigned long long s2 = atomicAdd(cursor + c2, 1ull), s3 = atomicAdd(cursor + c3, 1ull);
-            t_indices[s0] = r; t_data[s0] = v0;
-            t_indices[s1] = r; t_data[s1] = v1;
-            t_indices[s2] = r; t_data[s2] = v2;
-            t_indices[s3] = r; t_data[s3] = v3;
+            store_entry<PAIRS>(t_indices, t_data, s0, r, v0);
+            store_entry<PAIRS>(t_indices, t_data, s1, r, v1);
+            store_entry<PAIRS>(t_indices, t_data, s2, r, v2);
+            store_entry<PAIRS>(t_indices, t_data, s3, r, v3);
         }
         for (; k < e; k += 32) {
             const int c = ld_stream(indices + k);
             const float v = ld_stream(data + k);
-            const unsigned long long slot = atomicAdd(cursor + c, 1ull);
-            t_indices[slot] = r;
-            t_data[slot] = v;
+            store_entry<PAIRS>(t_indices, t_data, atomicAdd(cursor + c, 1ull), r, v);
         }
     }
 }
 
-// Same scatter, but (row, value) is written as ONE 8-byte pair: one scattered store per non-zero instead of
-// two (the fill is bound by the rate of scattered L2 operations, not by bytes).
-__global__ void __launch_bounds__(256)
-transpose_fill_pairs_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                            const float* __restrict__ data, int64_t n_rows, int64_t row_offset,
-                            unsigned long long* cursor, int2* __restrict__ t_pairs) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
-    const int64_t n_warps = (int64_t)gridDim.x * 8;
-    for (int64_t row = warp; row < n_rows; row += n_warps) {
-        const int64_t s = __ldg(indptr + row), e = __ldg(indptr + row + 1);
-        const int32_t r = (int32_t)(row + row_offset);
-        int64_t k = s + lane;
-        for (; k + 96 < e; k += 128) {
-            const int c0 = ld_stream(indices + k), c1 = ld_stream(indices + k + 32);
-            const int c2 = ld_stream(indices + k + 64), c3 = ld_stream(indices + k + 96);
-            const float v0 = ld_stream(data + k), v1 = ld_stream(data + k + 32);
-            const float v2 = ld_stream(data + k + 64), v3 = ld_stream(data + k + 96);
-            const unsigned long long s0 = atomicAdd(cursor + c0, 1ull), s1 = atomicAdd(cursor + c1, 1ull);
-            const unsigned long long s2 = atomicAdd(cursor + c2, 1ull), s3 = atomicAdd(cursor + c3, 1ull);
-            t_pairs[s0] = make_int2(r, __float_as_int(v0));
-            t_pairs[s1] = make_int2(r, __float_as_int(v1));
-            t_pairs[s2] = make_int2(r, __float_as_int(v2));
-            t_pairs[s3] = make_int2(r, __float_as_int(v3));
-        }
-        for (; k < e; k += 32) {
-            const int c = ld_stream(indices + k);
-            const float v = ld_stream(data + k);
-            t_pairs[atomicAdd(cursor + c, 1ull)] = make_int2(r, __float_as_int(v));
-        }
-    }
+// the two atomic-cursor entry points: shared validation, cursors seeded from the scanned histogram, one warp per row
+template <bool PAIRS>
+static int launch_transpose_fill(const char* name, const int64_t* indptr, const int32_t* indices, const float* data,
+                                 int64_t n_rows, int32_t n_cols, int64_t row_offset, const int64_t* t_indptr,
+                                 int64_t* cursor, int32_t* t_indices, float* t_data, mub_stream_t stream) {
+    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "%s: negative shape", name);
+    if (n_rows == 0 || n_cols == 0) return 0;
+    MUB_REQUIRE(indptr && t_indptr && cursor && t_indices && (PAIRS || t_data), "%s: null pointer", name);
+    MUB_REQUIRE(!PAIRS || ((uintptr_t)t_indices & 7) == 0, "%s: t_pairs must be 8-byte aligned", name);
+    cudaStream_t s = (cudaStream_t)stream;
+    copy_i64_kernel<<<(n_cols + 255) / 256, 256, 0, s>>>(t_indptr, cursor, n_cols);
+    int64_t want = (n_rows + 7) / 8;
+    int64_t cap = (int64_t)sm_count() * 8;
+    int grid = (int)(want < cap ? want : cap);
+    if (grid < 1) grid = 1;
+    transpose_fill_kernel<PAIRS><<<grid, 256, 0, s>>>(indptr, indices, data, n_rows, row_offset,
+                                                     (unsigned long long*)cursor, t_indices, t_data);
+    return check_launch(name);
 }
 
 // ---- tiled fill: no global atomics, deterministic ------------------------------------------------------------
@@ -367,19 +367,8 @@ extern "C" {
 int mub_csr_transpose_fill_pairs(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
                                  int32_t n_cols, int64_t row_offset, const int64_t* t_indptr, int64_t* cursor,
                                  int32_t* t_pairs, mub_stream_t stream) {
-    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "transpose_fill_pairs: negative shape");
-    if (n_rows == 0 || n_cols == 0) return 0;
-    MUB_REQUIRE(indptr && t_indptr && cursor && t_pairs, "transpose_fill_pairs: null pointer");
-    MUB_REQUIRE(((uintptr_t)t_pairs & 7) == 0, "transpose_fill_pairs: t_pairs must be 8-byte aligned");
-    cudaStream_t s = (cudaStream_t)stream;
-    mub::copy_i64_kernel<<<(n_cols + 255) / 256, 256, 0, s>>>(t_indptr, cursor, n_cols);
-    int64_t want = (n_rows + 7) / 8;
-    int64_t cap = (int64_t)mub::sm_count() * 8;
-    int grid = (int)(want < cap ? want : cap);
-    if (grid < 1) grid = 1;
-    mub::transpose_fill_pairs_kernel<<<grid, 256, 0, s>>>(indptr, indices, data, n_rows, row_offset,
-                                                         (unsigned long long*)cursor, (int2*)t_pairs);
-    return mub::check_launch("transpose_fill_pairs");
+    return mub::launch_transpose_fill<true>("transpose_fill_pairs", indptr, indices, data, n_rows, n_cols, row_offset,
+                                            t_indptr, cursor, t_pairs, nullptr, stream);
 }
 
 int mub_csrp_row_stats_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, double* sum, double* sumsq,
@@ -414,18 +403,8 @@ int mub_csr_transpose_count(const int32_t* indices, int64_t nnz, int32_t n_cols,
 int mub_csr_transpose_fill(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
                            int32_t n_cols, int64_t row_offset, const int64_t* t_indptr, int64_t* cursor,
                            int32_t* t_indices, float* t_data, mub_stream_t stream) {
-    MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "transpose_fill: negative shape");
-    if (n_rows == 0 || n_cols == 0) return 0;
-    MUB_REQUIRE(indptr && t_indptr && cursor && t_indices && t_data, "transpose_fill: null pointer");
-    cudaStream_t s = (cudaStream_t)stream;
-    mub::copy_i64_kernel<<<(n_cols + 255) / 256, 256, 0, s>>>(t_indptr, cursor, n_cols);
-    int64_t want = (n_rows + 7) / 8;
-    int64_t cap = (int64_t)mub::sm_count() * 8;
-    int grid = (int)(want < cap ? want : cap);
-    if (grid < 1) grid = 1;
-    mub::transpose_fill_kernel<<<grid, 256, 0, s>>>(indptr, indices, data, n_rows, row_offset,
-                                                   (unsigned long long*)cursor, t_indices, t_data);
-    return mub::check_launch("transpose_fill");
+    return mub::launch_transpose_fill<false>("transpose_fill", indptr, indices, data, n_rows, n_cols, row_offset,
+                                             t_indptr, cursor, t_indices, t_data, stream);
 }
 
 }  // extern "C"

@@ -322,8 +322,8 @@ def test_interleaved_masked_view_at_scale_matches_host_path(cuda):
     np.testing.assert_allclose(elbos[0], elbos[1], rtol=1e-5)
 
 
-# ---- shard position, float64 views, the tiled switch ---------------------------------------------------------------
-def test_selection_of_every_row_keeps_the_shard_position(cuda, monkeypatch):
+# ---- shard position, float64 views, unsorted sources ---------------------------------------------------------------
+def test_selection_keeps_the_shard_position_and_unsorted_sources_get_no_counts(cuda):
     X = _source(seed=5)
     A = mu.DeviceCSR.from_scipy(X)
     A.row0, A._n_total = 4000, 9000                      # rows [4000, 5500) of a 9000-cell matrix sharded over ranks
@@ -333,11 +333,11 @@ def test_selection_of_every_row_keeps_the_shard_position(cuda, monkeypatch):
         assert (out.row0, out.n_total) == (4000, 9000)
     part = _device.csr_select(A, np.arange(10, 20), mask)
     assert (part.row0, part.n_total) == (0, 10)
-    # MUON_B200_TFIDF_TILED=0 turns the tiled reduce pass off here too: no counts, the atomic-cursor fill
-    monkeypatch.setenv("MUON_B200_TFIDF_TILED", "0")
-    plain = _device.csr_select(A, None, mask)
+    # a shard not marked sorted gets no tiled reduce pass: no counts, the atomic-cursor fill
+    U = mu.DeviceCSR(A.indptr, A.indices, A.data, A.shape, row0=A.row0, n_total=A._n_total, sorted_indices=False)
+    plain = _device.csr_select(U, None, mask)
     assert "rb_counts" not in (getattr(plain, "_aux", None) or {}) and plain.transpose_panels(64).tiled_fill is False
-    _assert_same(plain, _expect(X, None, mask), "tiled pass off")
+    _assert_same(plain, _expect(X, None, mask), "unsorted source")
 
 
 def test_use_var_on_a_cell_shard_fits_as_the_premasked_shard(cuda):

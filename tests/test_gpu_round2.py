@@ -196,8 +196,11 @@ def test_host_path_pipeline_blocks_and_twin_validation(cuda, monkeypatch):
     """tfidf() on a host matrix: several upload/download blocks, int64 and int32 host indices, result equal to the
     one-shot device path bit for bit; the device twin is reused by lsi() only while EVERY host element is intact."""
     monkeypatch.setattr(_device, "_BLOCK_NNZ", 50_000)
+    monkeypatch.setattr(_device.TransposedPanels, "L2_BUDGET", 1 << 17)       # 512 cells per panel at pad 64
     C = generate_host(3000, 900, 0.05, n_topics=8, seed=4)
-    ref = _device.tfidf_csr(mu.DeviceCSR.from_scipy(C)).get()
+    dref = _device.tfidf_csr(mu.DeviceCSR.from_scipy(C))
+    ref = dref.get()
+    Tref = _device.TransposedPanels(dref, 64)
     for idt in (np.int32, np.int64):
         X = sp.csr_matrix(C.shape, dtype=np.float32)
         X.data, X.indices, X.indptr = C.data.copy(), C.indices.astype(idt), C.indptr.astype(idt)
@@ -206,7 +209,17 @@ def test_host_path_pipeline_blocks_and_twin_validation(cuda, monkeypatch):
         assert ad.X.indices.dtype == idt and ad.X.indices is X.indices      # replaces its source: arrays shared
         np.testing.assert_array_equal(ad.X.data, ref.data)
         assert len(getattr(ad.X, _device._RESIDENT_ATTR)[1]["blocks"]) >= 3
-        assert _device.recall_resident(ad.X) is not None
+        twin = _device.recall_resident(ad.X)
+        assert twin is not None
+        # entry counts taken block by block (each block at its own rows) == those of the one-shot device path, and
+        # so are the transposed panels built from them
+        assert twin._aux["col_counts"][0] == dref._aux["col_counts"][0]
+        assert torch.equal(twin._aux["col_counts"][1], dref._aux["col_counts"][1])
+        assert torch.equal(twin._aux["rb_counts"], dref._aux["rb_counts"])
+        T = _device.TransposedPanels(twin, 64)
+        assert T.tiled_fill and Tref.tiled_fill and len(T.panels) == len(Tref.panels) >= 4
+        for (a0, a1, Pa), (b0, b1, Pb) in zip(T.panels, Tref.panels):
+            assert (a0, a1) == (b0, b1) and torch.equal(Pa.indptr, Pb.indptr) and torch.equal(Pa.pairs, Pb.pairs)
         # (a) one value edited, (b) two values swapped, (c) one column index edited, (d) indptr edited
         v = ad.X.data[1234]
         ad.X.data[1234] = v * 1.5
@@ -255,7 +268,7 @@ def test_host_path_pipeline_blocks_and_twin_validation(cuda, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------------
-def test_tiled_reduce_equals_atomic_reduce_and_counts_feed_the_transposition(cuda, monkeypatch):
+def test_tiled_reduce_equals_atomic_reduce_of_unsorted_input_and_counts_feed_the_transposition(cuda, monkeypatch):
     """The shared-memory tiled reduce pass: row sums / column sums bit-identical to the one-atomic-per-non-zero
     kernel (integer-valued counts: every order gives the same fp32 sum), entry counts per (row chunk, column)
     equal to a bincount, panels built from those counts identical to panels built by the counting pass, and the
@@ -264,9 +277,9 @@ def test_tiled_reduce_equals_atomic_reduce_and_counts_feed_the_transposition(cud
     C = generate_host(5000, 30000, 0.03, n_topics=8, seed=9)         # 3 column tiles, 10 row blocks
     A = mu.DeviceCSR.from_scipy(C)
     n, d = C.shape
-    monkeypatch.setenv("MUON_B200_TFIDF_TILED", "0")
-    ref = _device.tfidf_csr(A)
-    monkeypatch.setenv("MUON_B200_TFIDF_TILED", "1")
+    # the same arrays not marked sorted take the order-agnostic kernel, which leaves no counts
+    unsorted = lambda: mu.DeviceCSR(A.indptr, A.indices, A.data, A.shape, sorted_indices=False)  # noqa: E731
+    ref = _device.tfidf_csr(unsorted())
     got = _device.tfidf_csr(A)
     for key in ("row_sum", "col_sum", "idf"):
         assert torch.equal(ref._aux[key], got._aux[key]), key
@@ -279,7 +292,6 @@ def test_tiled_reduce_equals_atomic_reduce_and_counts_feed_the_transposition(cud
         assert np.array_equal(counts[c].cpu().numpy(), want), c
     # transposed panels from the reused counts == panels from the counting pass (same indptr; same entry SETS per row)
     monkeypatch.setattr(_device.TransposedPanels, "L2_BUDGET", 1 << 18)       # 1024 cells per panel at pad 64 -> 8 panels
-    monkeypatch.setenv("MUON_B200_FILL_TILED", "1")             # the deterministic tiled fill (default)
     Tp = _device.TransposedPanels(got, 64)
     Tq = _device.TransposedPanels(ref, 64)
     assert Tp.counts_reused and Tp.tiled_fill and not Tq.counts_reused and not Tq.tiled_fill
@@ -291,8 +303,9 @@ def test_tiled_reduce_equals_atomic_reduce_and_counts_feed_the_transposition(cud
         rows = torch.repeat_interleave(torch.arange(d, device=cuda), Ta.indptr[1:] - Ta.indptr[:-1])
         key = rows * (1 << 20) + Ta.pairs[:, 0].to(torch.int64)
         assert bool((key[1:] > key[:-1]).all())
-    monkeypatch.setenv("MUON_B200_FILL_TILED", "0")
-    Tr = _device.TransposedPanels(got, 64)                       # reused counts, atomic-cursor fill
+    got_cc = got.with_data(got.data)                             # the per-chunk counts only, no per-block counts
+    got_cc._aux = {"col_counts": got._aux["col_counts"]}
+    Tr = _device.TransposedPanels(got_cc, 64)                    # reused counts, atomic-cursor fill
     assert Tr.counts_reused and not Tr.tiled_fill
     for (a0, a1, Ta), (b0, b1, Tb) in zip(Tp.panels, Tr.panels):
         # same ENTRIES per transposed row ((peak, cell) is unique): order by (peak, cell) and compare cells and value bits
@@ -310,10 +323,8 @@ def test_tiled_reduce_equals_atomic_reduce_and_counts_feed_the_transposition(cud
         assert np.abs(ya - yb).max() <= 1e-5 * np.abs(yb).max()       # same entry sets, different summation order
     # binarize fused, float sums exact
     gb = _device.tfidf_csr(A, binarize=True)
-    monkeypatch.setenv("MUON_B200_TFIDF_TILED", "0")
-    rb = _device.tfidf_csr(A, binarize=True)
+    rb = _device.tfidf_csr(unsorted(), binarize=True)
     assert torch.equal(gb.data, rb.data)
-    monkeypatch.setenv("MUON_B200_TFIDF_TILED", "1")
     # an unsorted row: flagged (check_canonical) / silently handled by the order-agnostic kernel (device input)
     Xu = C.copy()
     a = Xu.indptr[777]

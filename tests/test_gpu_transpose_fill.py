@@ -59,7 +59,6 @@ def test_tiled_fill_is_the_transpose(cuda, monkeypatch, n, d, density, budget):
     X = sp.csr_matrix((got.data.cpu().numpy(), C.indices, C.indptr), shape=C.shape)
     if budget is not None:
         monkeypatch.setattr(_device.TransposedPanels, "L2_BUDGET", budget)
-    monkeypatch.setenv("MUON_B200_FILL_TILED", "1")
     T = _device.TransposedPanels(got, 64)
     assert T.counts_reused and T.tiled_fill and len(T.panels) >= 2
     _assert_panels_are_the_transpose(T, X)
@@ -72,7 +71,6 @@ def test_tiled_fill_falls_back_when_the_pattern_changed(cuda, monkeypatch):
     C = _edge_matrix(5000, 30000, 0.02, seed=11)
     got = _device.tfidf_csr(mu.DeviceCSR.from_scipy(C))
     monkeypatch.setattr(_device.TransposedPanels, "L2_BUDGET", 1 << 18)
-    monkeypatch.setenv("MUON_B200_FILL_TILED", "1")
     assert _device.TransposedPanels(got, 64).tiled_fill
     # (1) per-block counts moved between two blocks of one panel: the column totals still agree with t_indptr,
     # only the fill itself can see that block 0 holds a different number of entries
