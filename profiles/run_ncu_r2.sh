@@ -11,5 +11,4 @@ timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -c 2500 --
 timeout 600 ncu --set full --clock-control none --import-source on -k regex:"tfidf_reduce_tiled|tfidf_apply|transpose_fill_pairs" -c 3 -o $O/prof_tfidf -f $B > $O/ncu_tfidf.log 2>&1
 # the default LSI schedule starts with half-operand passes, so the first SpMM launches are the half instantiations
 timeout 600 ncu --set full --clock-control none --import-source on -k regex:"rowwarp_kernel" -c 3 -o $O/prof_spmm_half -f $B > $O/ncu_half.log 2>&1
-MUON_B200_LSI_LOWP_TOL=0 timeout 600 ncu --set full --clock-control none --import-source on -k regex:"rowwarp_kernel" -c 3 -o $O/prof_spmm_f32 -f $B > $O/ncu_f32.log 2>&1
 ls -la $O

@@ -96,21 +96,18 @@ def test_no_cpu_fallback():
 
 
 @pytest.mark.parametrize("k,P", [(8, 32), (20, 32), (30, 64)])
-def test_block_lanczos_matches_svds(k, P):
+def test_block_lanczos_ritz_triplets_from_the_left_blocks_match_svds(k, P):
+    """U_k read off the stored left Lanczos blocks, s and V_k meet the float64 svds parity bar, and U_k is
+    orthonormal."""
     X = tfidf_ref(generate_host(1500, 1200, 0.05, n_topics=12, seed=3)).astype(np.float32)
     ref = lsi_ref(X, k + 1, dtype=np.float64)
     s_next = ref["svalues"][k]
     ref = {"svalues": ref["svalues"][:k], "U": ref["U"][:, :k], "LSI": ref["LSI"][:, :k]}
-    U, s, V, info = truncated_svd(ScipyOperator(X), k, P, tol=1e-5, polish=True)
+    U, s, V, info = truncated_svd(ScipyOperator(X), k, P, tol=1e-5)
     assert info.converged
     out = compare_lsi({"svalues": s.numpy(), "U": U.numpy(), "LSI": V.numpy()}, ref, rtol=1e-4, s_next=s_next)
     assert out["sigma_rel"] < 1e-5
-    # without the final Rayleigh-Ritz pass (the default): same accuracy from the Krylov spaces alone, one pass fewer
-    U2, s2, V2, info2 = truncated_svd(ScipyOperator(X), k, P, tol=1e-5, polish=False)
-    assert info2.passes == info.passes - 1 and U2.shape == U.shape
-    out2 = compare_lsi({"svalues": s2.numpy(), "U": U2.numpy(), "LSI": V2.numpy()}, ref, rtol=1e-4, s_next=s_next)
-    assert out2["sigma_rel"] < 1e-5
-    assert np.abs(U2.numpy().T.astype(np.float64) @ U2.numpy() - np.eye(k)).max() < 1e-5
+    assert np.abs(U.numpy().T.astype(np.float64) @ U.numpy() - np.eye(k)).max() < 1e-5
 
 
 def test_block_lanczos_small_dims_and_restart():
@@ -218,12 +215,18 @@ def test_neighbors_argument_errors_and_no_cpu_fallback():
 
 class HalfOperandOperator(ScipyOperator):
     """ScipyOperator that also offers the product's low-precision mode: the dense operand of a product is rounded
-    to IEEE half after the same power-of-two scaling the CUDA path uses (muon_b200._device.HALF_SCALE)."""
+    to IEEE half after the same power-of-two scaling the CUDA path uses (muon_b200._device.HALF_SCALE).  Like
+    CsrOperator it has gram_local, so the driver's d-space QR is CholeskyQR2."""
     lowp = True
 
     def __init__(self, A):
         super().__init__(A)
         self.lowp_calls = 0
+        self.gram_local_calls = 0
+
+    def gram_local(self, Y, l):
+        self.gram_local_calls += 1
+        return self.gram(Y, l)
 
     @staticmethod
     def _round(M):
@@ -238,8 +241,8 @@ class HalfOperandOperator(ScipyOperator):
         return torch.from_numpy(self.At @ (self._round(Y) if lowp else Y.numpy()))
 
 
-@pytest.mark.parametrize("k,P,polish", [(20, 32, True), (30, 64, False)])
-def test_block_lanczos_half_precision_phase(k, P, polish):
+@pytest.mark.parametrize("k,P", [(20, 32), (30, 64)])
+def test_block_lanczos_half_precision_phase(k, P):
     """Two-phase schedule: half-precision operands until 1e-3, then fp32 from the Ritz vectors.  The result must
     meet the same parity bar as the all-fp32 iteration, with most passes done in the cheap mode."""
     X = tfidf_ref(generate_host(1500, 1200, 0.05, n_topics=12, seed=3)).astype(np.float32)
@@ -247,13 +250,13 @@ def test_block_lanczos_half_precision_phase(k, P, polish):
     s_next = ref["svalues"][k]
     ref = {"svalues": ref["svalues"][:k], "U": ref["U"][:, :k], "LSI": ref["LSI"][:, :k]}
     op = HalfOperandOperator(X)
-    U, s, V, info = truncated_svd(op, k, P, tol=1e-5, lowp_tol=1e-3, polish=polish)
-    assert info.converged and info.lowp_passes == op.lowp_calls > 0
+    U, s, V, info = truncated_svd(op, k, P, tol=1e-5)
+    assert info.converged and info.lowp_passes == op.lowp_calls > 0 and op.gram_local_calls > 0
     assert info.lowp_passes >= info.passes // 2, (info.lowp_passes, info.passes)
     out = compare_lsi({"svalues": s.numpy(), "U": U.numpy(), "LSI": V.numpy()}, ref, rtol=1e-4, s_next=s_next)
     assert out["sigma_rel"] < 1e-5
-    # an operator without the low-precision mode ignores the request
-    U2, s2, V2, info2 = truncated_svd(ScipyOperator(X), k, P, tol=1e-5, lowp_tol=1e-3)
+    # an operator without the low-precision mode runs fp32 only
+    U2, s2, V2, info2 = truncated_svd(ScipyOperator(X), k, P, tol=1e-5)
     assert info2.lowp_passes == 0
 
 
@@ -289,7 +292,7 @@ def test_reference_arm_does_not_load_the_cuda_library():
     assert '"impl": "reference"' in out.stdout
 
 
-def test_sampled_residual_check_saves_the_confirming_pass():
+def test_sampled_residual_check_replaces_only_the_confirming_pass():
     """When the history predicts convergence the driver estimates the residual on a sample of the peaks and skips the
     pass that would only confirm it; the result meets the same parity bar, an operator without the hook is unaffected,
     and a failed estimate falls through to the full pass."""
@@ -298,9 +301,9 @@ def test_sampled_residual_check_saves_the_confirming_pass():
     ref = lsi_ref(X, k + 1, dtype=np.float64)
     s_next = ref["svalues"][k]
     ref = {"svalues": ref["svalues"][:k], "U": ref["U"][:, :k], "LSI": ref["LSI"][:, :k]}
-    U0, s0, V0, info0 = truncated_svd(ScipyOperator(X), k, P, tol=1e-5, polish=False)
+    U0, s0, V0, info0 = truncated_svd(ScipyOperator(X), k, P, tol=1e-5)
     op = SamplingOperator(X)
-    U, s, V, info = truncated_svd(op, k, P, tol=1e-5, polish=False)
+    U, s, V, info = truncated_svd(op, k, P, tol=1e-5)
     assert info0.sampled_checks == 0 and op.samples == info.sampled_checks >= 1
     if info.sampled_stop:
         assert info.passes == info0.passes - 1
@@ -313,7 +316,7 @@ def test_sampled_residual_check_saves_the_confirming_pass():
             return super().residual_sample(Uk, Vk, sig) * 1e3          # never accepted
 
     op2 = Pessimist(X)
-    U2, s2, V2, info2 = truncated_svd(op2, k, P, tol=1e-5, polish=False)
+    U2, s2, V2, info2 = truncated_svd(op2, k, P, tol=1e-5)
     assert not info2.sampled_stop and info2.passes == info0.passes and info2.converged
     np.testing.assert_allclose(s2.numpy(), s0.numpy(), rtol=1e-6)
 
