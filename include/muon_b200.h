@@ -94,10 +94,17 @@ int mub_tfidf_apply_f64(const int64_t* indptr, const int32_t* indices, const dou
  * Y^T Z / Y W contractions of mofapy2 (called from muon/_core/tools.py:583-585).
  * ld in {32,64,128}.  accumulate: 0 -> C = A*B, 1 -> C += A*B.
  * row_counter: optional device int64 scratch word, zeroed by the caller, enabling dynamic row
- * scheduling (recommended for skewed row lengths, e.g. transposed ATAC matrices); may be NULL. */
+ * scheduling (recommended for skewed row lengths, e.g. transposed ATAC matrices); may be NULL.
+ * flags: MUB_SPMM_ROWS_SORTED states that every row's column indices are ascending (a caller
+ * promise, not checked: unsorted rows then give wrong results).  mub_spmm_csr_f32 then runs the
+ * tiled kernel, which stages B in shared memory in column tiles once per band of 128 rows instead
+ * of gathering a row of B from L2 per non-zero (row_counter is then unused).  The other three
+ * entry points accept the flag and keep the row-warp kernel.  Both kernels return the same bits. */
+#define MUB_SPMM_ROWS_SORTED 1u
 int mub_spmm_csr_f32(const int64_t* indptr, const int32_t* indices, const float* data,
                      int64_t n_rows, int64_t n_cols, const float* B, int32_t ld, float* C,
-                     int32_t accumulate, unsigned long long* row_counter, mub_stream_t stream);
+                     int32_t accumulate, unsigned long long* row_counter, uint32_t flags,
+                     mub_stream_t stream);
 
 /* ---- CSR transpose (one-time per matrix): builds the CSR of A^T so that A^T * Y is again a
  * row-gather SpMM (scipy does the same implicitly through csc_matvec, _svds.py:447).
@@ -133,7 +140,7 @@ int mub_csr_transpose_fill_tiled(const int64_t* indptr, const int32_t* indices, 
                                  int32_t* t_pairs, int32_t* status, mub_stream_t stream);
 int mub_spmm_csrp_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, int64_t n_cols,
                       const float* B, int32_t ld, float* C, int32_t accumulate, unsigned long long* row_counter,
-                      mub_stream_t stream);
+                      uint32_t flags, mub_stream_t stream);
 int mub_csrp_row_stats_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, double* sum,
                            double* sumsq, mub_stream_t stream);
 
@@ -283,10 +290,10 @@ int mub_wnn_affinity_topk_f32(int32_t n_mod, const float* const* reps, const int
 int mub_f32_to_f16_scaled(const float* src, int64_t n, float scale, void* dst, mub_stream_t stream);
 int mub_spmm_csr_h16(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
                      int64_t n_cols, const void* B_half, int32_t ld, float* C, int32_t accumulate,
-                     float out_scale, unsigned long long* row_counter, mub_stream_t stream);
+                     float out_scale, unsigned long long* row_counter, uint32_t flags, mub_stream_t stream);
 int mub_spmm_csrp_h16(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, int64_t n_cols,
                       const void* B_half, int32_t ld, float* C, int32_t accumulate, float out_scale,
-                      unsigned long long* row_counter, mub_stream_t stream);
+                      unsigned long long* row_counter, uint32_t flags, mub_stream_t stream);
 
 /* ---- host <-> device staging (ingest side: adata.X is a pageable scipy CSR, muon/_atac/preproc.py:86-129
  * reads it and rebinds a freshly allocated host matrix).  A stager owns a ring of pinned buffers and a pool

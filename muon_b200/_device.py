@@ -12,8 +12,8 @@ import numpy as np
 import torch
 
 from . import _dist
-from ._lib import (TFIDF_BINARIZE, TFIDF_LOG_IDF, TFIDF_LOG_TF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE, MuonB200Error, call, load, ptr,
-                   stream_ptr)
+from ._lib import (SPMM_ROWS_SORTED, TFIDF_BINARIZE, TFIDF_LOG_IDF, TFIDF_LOG_TF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE,
+                   MuonB200Error, call, load, ptr, stream_ptr)
 
 PAD_WIDTHS = (32, 64, 128)
 
@@ -320,7 +320,8 @@ class DeviceCSR:
         if dtype is None:
             dtype = np.float32 if data.dtype == np.float32 else (np.float64 if data.dtype == np.float64 else np.float32)
         return cls(to_device(X.indptr, device, np.int64), to_device(X.indices, device, np.int32),
-                   to_device(data, device, dtype), X.shape)
+                   to_device(data, device, dtype), X.shape,
+                   sorted_indices=bool(getattr(X, "has_sorted_indices", False)))
 
     @classmethod
     def from_scipy_shard(cls, X, world: Optional[int] = None, rank: Optional[int] = None, device=None) -> "DeviceCSR":
@@ -370,12 +371,12 @@ class DeviceCSR:
 class DevicePairs:
     """CSR whose entries are interleaved 8-byte {int32 index, float32 value} pairs (``pairs``: int32 [nnz, 2]).
     Used for the transposed row panels: one scattered store per non-zero when building, one 8-byte load per
-    entry when multiplying."""
+    entry when multiplying.  ``sorted_indices``: every row lists its columns in ascending order."""
 
-    def __init__(self, indptr, pairs, shape):
+    def __init__(self, indptr, pairs, shape, sorted_indices: bool = False):
         self.indptr, self.pairs = indptr, pairs
         self.shape = (int(shape[0]), int(shape[1]))
-        self.sorted_indices = False
+        self.sorted_indices = sorted_indices
 
     @property
     def nnz(self) -> int:
@@ -690,7 +691,8 @@ class TransposedPanels:
             cursor = torch.empty(max(d, 1), dtype=torch.int64, device=dev)
             call("mub_csr_transpose_fill_pairs", ptr(A.indptr) + 8 * r0, ptr(A.indices), ptr(A.data), r1 - r0, d, 0,
                  ptr(t_indptr), ptr(cursor), ptr(t_pairs), st)
-        return r0, r1, DevicePairs(t_indptr, t_pairs, (d, r1 - r0))
+        # the tiled fill lists every transposed row in ascending cell order (it is only kept if its status is clear)
+        return r0, r1, DevicePairs(t_indptr, t_pairs, (d, r1 - r0), sorted_indices=tiled is not None)
 
     def spmm(self, Y: torch.Tensor, dynamic=True, half: bool = False) -> torch.Tensor:
         """A^T Y accumulated panel by panel.  ``half``: round Y to IEEE half first (see ``spmm``)."""
@@ -756,22 +758,27 @@ def spmm(A, B: torch.Tensor, out: Optional[torch.Tensor] = None, accumulate=Fals
          scale: float = HALF_SCALE) -> torch.Tensor:
     """K2/K3: C[n x P] (+)= A @ B[d x P];  P = B.shape[1] must be 32, 64 or 128.  A is a ``DeviceCSR`` or
     ``DevicePairs``.  B is float32, or float16 holding B * ``scale`` (``to_half_scaled``): half the bytes per non-zero
-    through the L2 -> L1 gather path that bounds the fp32 operand; products and sums stay fp32."""
+    through the L2 -> L1 gather path that bounds the fp32 operand; products and sums stay fp32.  A matrix whose rows
+    are sorted (``A.sorted_indices``) is flagged so to the library, which then runs a fp32 product on CSR arrays with
+    the tiled kernel (B staged in shared memory); everything else takes the row-warp kernel (``dynamic``: rows claimed
+    from an atomic counter).  Both give the same bits."""
     n, d = A.shape
     P = B.shape[1]
     assert B.shape[0] == d and B.dtype in (torch.float32, torch.float16) and B.is_contiguous(), (B.shape, d, B.dtype)
     if out is None:
         assert not accumulate
         out = torch.empty((n, P), dtype=torch.float32, device=B.device)
+    flags = SPMM_ROWS_SORTED if A.sorted_indices else 0
     counter = torch.zeros(1, dtype=torch.int64, device=B.device) if dynamic else None
     j0, j1, o0 = _row_range(rows, n)                    # matrix rows [j0, j1) -> out rows [o0, o0 + j1 - j0)
     pairs = isinstance(A, DevicePairs)
     operands = [ptr(A.indptr) + 8 * j0] + ([ptr(A.pairs)] if pairs else [ptr(A.indices), ptr(A.data)])
     operands += [j1 - j0, d, ptr(B), P, ptr(out) + 4 * P * o0, 1 if accumulate else 0]
     if B.dtype == torch.float16:
-        call("mub_spmm_csrp_h16" if pairs else "mub_spmm_csr_h16", *operands, 1.0 / scale, ptr(counter), stream_ptr())
+        call("mub_spmm_csrp_h16" if pairs else "mub_spmm_csr_h16", *operands, 1.0 / scale, ptr(counter), flags,
+             stream_ptr())
     else:
-        call("mub_spmm_csrp_f32" if pairs else "mub_spmm_csr_f32", *operands, ptr(counter), stream_ptr())
+        call("mub_spmm_csrp_f32" if pairs else "mub_spmm_csr_f32", *operands, ptr(counter), flags, stream_ptr())
     return out
 
 

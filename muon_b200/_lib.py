@@ -33,12 +33,12 @@ SIGNATURES = {
     "mub_tfidf_idf_f64": [vp, i32, f64, u32, vp, vp],
     "mub_tfidf_apply_f32": [vp, vp, vp, vp, i64, i32, vp, vp, f32, u32, vp],
     "mub_tfidf_apply_f64": [vp, vp, vp, vp, i64, i32, vp, vp, f64, u32, vp],
-    "mub_spmm_csr_f32": [vp, vp, vp, i64, i64, vp, i32, vp, i32, vp, vp],
+    "mub_spmm_csr_f32": [vp, vp, vp, i64, i64, vp, i32, vp, i32, vp, u32, vp],
     "mub_csr_transpose_count": [vp, i64, i32, vp, vp],
     "mub_csr_transpose_fill": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp, vp],
     "mub_gram_f32": [vp, vp, i64, i32, i32, vp, vp, vp],
     "mub_csr_transpose_fill_pairs": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp],
-    "mub_spmm_csrp_f32": [vp, vp, i64, i64, vp, i32, vp, i32, vp, vp],
+    "mub_spmm_csrp_f32": [vp, vp, i64, i64, vp, i32, vp, i32, vp, u32, vp],
     "mub_csrp_row_stats_f32": [vp, vp, i64, vp, vp, vp],
     "mub_csr_select_count": [vp, vp, i64, i32, vp, i64, vp, vp, vp],
     "mub_csr_select_fill_f32": [vp, vp, vp, i32, vp, i64, vp, vp, vp, vp, vp],
@@ -56,8 +56,8 @@ SIGNATURES = {
     "mub_wnn_bandwidth_f32": [vp, vp, vp, vp, vp, i64, i32, i32, i32, f64, vp, vp, vp, i64, vp, i32, i32, vp],
     "mub_wnn_affinity_topk_f32": [i32, vp, vp, vp, vp, vp, vp, i64, i32, i32, vp, vp, vp, vp],
     "mub_f32_to_f16_scaled": [vp, i64, f32, vp, vp],
-    "mub_spmm_csr_h16": [vp, vp, vp, i64, i64, vp, i32, vp, i32, f32, vp, vp],
-    "mub_spmm_csrp_h16": [vp, vp, i64, i64, vp, i32, vp, i32, f32, vp, vp],
+    "mub_spmm_csr_h16": [vp, vp, vp, i64, i64, vp, i32, vp, i32, f32, vp, u32, vp],
+    "mub_spmm_csrp_h16": [vp, vp, i64, i64, vp, i32, vp, i32, f32, vp, u32, vp],
     "mub_stager_create": [C.c_size_t, i32, i32, C.POINTER(vp)],
     "mub_stager_destroy": [vp],
     "mub_stager_h2d": [vp, vp, vp, C.c_size_t, i32, i32, C.POINTER(u64), C.POINTER(i32), vp],
@@ -76,6 +76,7 @@ SPECIAL_RESTYPE = {
 }
 
 TFIDF_LOG_TF, TFIDF_LOG_IDF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE, TFIDF_BINARIZE = 1, 2, 4, 8, 16
+SPMM_ROWS_SORTED = 1
 
 
 class MuonB200Error(RuntimeError):

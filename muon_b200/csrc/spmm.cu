@@ -16,6 +16,14 @@
 // Traffic model (DESIGN.md): HBM streams 8 B/nnz (+ dense operands once); every non-zero
 // additionally pulls P * sizeof(T) bytes of B through L2->L1, which is the practical limiter at P>=32.
 //
+// "Tiled" kernel, for CSR arrays whose rows are known to be sorted by column and the fp32 operand: a CTA owns a band of kTiledRows consecutive rows and sweeps
+// B in column tiles (TC consecutive rows of B, one contiguous slab), each staged once into shared memory by a 1-D
+// bulk copy (TMA) and shared by every row of the band.  Each operand row then leaves L2 once per band instead of once
+// per non-zero, and the gathers are served from shared memory.  A warp keeps W rows' accumulators in registers and
+// a 32-entry window of each row's (index, value) stream; the ballot of "column < tile end" over the window gives the
+// row's segment in the tile.  Entry q of a row goes to lane group q mod G in ascending q, as in the row-warp kernel,
+// and the butterfly and store are the same: both kernels return the same bits.
+//
 // Half operand: every non-zero gathers half the bytes of the fp32 kernel.  Products and sums are fp32
 // (half -> float conversion is exact), only the operand is rounded (2^-11 relative).  Used by the early
 // block-Lanczos steps of the LSI driver (_lsi.py), whose accuracy need not exceed 1e-3; the final steps
@@ -23,6 +31,7 @@
 // (mub_f32_to_f16_scaled).
 #include <cuda_fp16.h>
 
+#include <climits>
 #include <type_traits>
 
 #include "common.cuh"
@@ -58,6 +67,38 @@ __device__ __forceinline__ void fma_gather(float* acc, float v, const uint4& q) 
             const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
             acc[2 * i] = fmaf(v, f.x, acc[2 * i]);
             acc[2 * i + 1] = fmaf(v, f.y, acc[2 * i + 1]);
+        }
+    }
+}
+
+// combine the G lane groups of a row's partial sums (fixed butterfly order: deterministic) and store the row
+template <int P, typename T>
+__device__ __forceinline__ void store_row(float* acc, float* __restrict__ C_row, int accumulate, float out_scale,
+                                          int lane) {
+    constexpr int VEC = 16 / sizeof(T);
+    constexpr int LPN = P / VEC;
+    const int sub = lane % LPN, grp = lane / LPN;
+#pragma unroll
+    for (int off = LPN; off < 32; off <<= 1) {
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
+    }
+    if (grp == 0) {
+        float4* dst = reinterpret_cast<float4*>(C_row + sub * VEC);
+#pragma unroll
+        for (int j = 0; j < VEC / 4; ++j) {
+            float4 r = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+            if constexpr (std::is_same_v<T, __half>) {
+                // __fmul_rn is never contracted with the add below: the scaled product is rounded on its own, as it
+                // is without accumulate
+                r.x = __fmul_rn(r.x, out_scale); r.y = __fmul_rn(r.y, out_scale);
+                r.z = __fmul_rn(r.z, out_scale); r.w = __fmul_rn(r.w, out_scale);
+            }
+            if (accumulate) {
+                const float4 o = dst[j];
+                r.x += o.x; r.y += o.y; r.z += o.z; r.w += o.w;
+            }
+            dst[j] = r;
         }
     }
 }
@@ -117,30 +158,7 @@ __device__ __forceinline__ void spmm_row(const int32_t* __restrict__ indices, co
             if (src < cnt) fma_gather<T>(acc, vt, ld_gather_u4(Bl + (size_t)cc * P));
         }
     }
-    // combine the G lane groups (fixed butterfly order: deterministic)
-#pragma unroll
-    for (int off = LPN; off < 32; off <<= 1) {
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
-    }
-    if (grp == 0) {
-        float4* dst = reinterpret_cast<float4*>(C_row + sub * VEC);
-#pragma unroll
-        for (int j = 0; j < VEC / 4; ++j) {
-            float4 r = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-            if constexpr (std::is_same_v<T, __half>) {
-                // __fmul_rn is never contracted with the add below: the scaled product is rounded on its own, as it
-                // is without accumulate
-                r.x = __fmul_rn(r.x, out_scale); r.y = __fmul_rn(r.y, out_scale);
-                r.z = __fmul_rn(r.z, out_scale); r.w = __fmul_rn(r.w, out_scale);
-            }
-            if (accumulate) {
-                const float4 o = dst[j];
-                r.x += o.x; r.y += o.y; r.z += o.z; r.w += o.w;
-            }
-            dst[j] = r;
-        }
-    }
+    store_row<P, T>(acc, C_row, accumulate, out_scale, lane);
 }
 
 template <int P, bool PAIRS, typename T>
@@ -183,19 +201,220 @@ static int launch_spmm(const int64_t* indptr, const int32_t* indices, const floa
     return check_launch(name);
 }
 
-// the four C entry points: shared validation, then one instantiation per ld
+// ---- tiled kernel ------------------------------------------------------------------------------------------------
+// CSR arrays and the fp32 operand only (see spmm_entry).  16 warps x 8 rows = a band of 128 rows per CTA, one CTA per SM (512 threads, <= 128 registers
+// each: a row's partial sums are 4 registers per lane).  Two stages of kTiledStageBytes: TC = kTiledStageBytes / (4 P)
+// rows of B per tile.  The kernel's time is a fixed part plus a cost per (row, tile) segment, so the tiles are as tall
+// as two stages allow next to the L1 that caches the entry windows.
+constexpr int kTiledWarps = 16;
+constexpr int kTiledThreads = kTiledWarps * kWarp;
+constexpr int kTiledRowsPerWarp = 8;
+constexpr int kTiledRows = kTiledWarps * kTiledRowsPerWarp;
+constexpr int kTiledStages = 2;
+constexpr int kTiledStageBytes = 96 << 10;  // TC = 384 rows of B at P = 64: ~12 entries per segment at 3 % density
+constexpr int kTiledSmemBytes = kTiledStages * kTiledStageBytes;
+
+__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
+    asm volatile(
+        "{\n\t.reg .pred done;\n"
+        "WAIT_%=:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 done, [%0], %1;\n\t"
+        "@!done bra WAIT_%=;\n}" ::"r"(smem_addr(bar)), "r"(parity) : "memory");
+}
+// bytes of B[src, src + bytes) -> shared dst; completion is counted on bar
+__device__ __forceinline__ void tma_load_1d(void* dst, const void* src, unsigned bytes, uint64_t* bar) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)) : "memory");
+}
+
+// lane j <- entry pos + j of the row [start, start + len), column INT_MAX past the row's end.  Cached loads: the part
+// of the window a tile does not consume is read again at the next tile
+__device__ __forceinline__ void load_window(const int32_t* __restrict__ indices, const float* __restrict__ data,
+                                            int64_t start, int pos, int len, int lane, int& c, float& v) {
+    c = INT_MAX;
+    v = 0.f;
+    if (pos + lane < len) {
+        c = __ldg(indices + start + pos + lane);
+        v = __ldg(data + start + pos + lane);
+    }
+}
+
+// window lanes [0, cnt) hold row entries pos .. pos + cnt - 1, all in the staged tile (first row of B: lo):
+// entry q goes to lane group q mod G, in ascending q
+template <int P, typename T>
+__device__ __forceinline__ void gather_segment(float* acc, const T* __restrict__ tile, int lo, int c, float v, int pos,
+                                               int cnt, int lane) {
+    constexpr int VEC = 16 / sizeof(T);
+    constexpr int LPN = P / VEC;
+    constexpr int G = 32 / LPN;
+    constexpr int BATCH = 4;  // gathers in flight per lane (a segment is ~0.03 * TC / G ~ 4 gathers)
+    const int sub = lane % LPN;
+    const int first = ((lane / LPN) - pos) & (G - 1);  // this group's first window lane
+    const T* tl = tile + sub * VEC;
+    for (int k0 = 0; k0 < cnt; k0 += BATCH * G) {  // warp-uniform trip count: the loop holds shuffles
+        uint4 b[BATCH];
+        float vv[BATCH];
+#pragma unroll
+        for (int t = 0; t < BATCH; ++t) {
+            const int j = k0 + t * G + first;
+            const int cc = __shfl_sync(0xffffffffu, c, j & 31);
+            vv[t] = __shfl_sync(0xffffffffu, v, j & 31);
+            if (j < cnt) b[t] = *reinterpret_cast<const uint4*>(tl + (cc - lo) * P);
+        }
+#pragma unroll
+        for (int t = 0; t < BATCH; ++t)
+            if (k0 + t * G + first < cnt) fma_gather<T>(acc, vv[t], b[t]);
+    }
+}
+
+template <int P>
+__global__ void __launch_bounds__(kTiledThreads, 1)
+spmm_csr_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                      const float* __restrict__ data, int64_t n_rows, int n_cols, const float* __restrict__ B,
+                      float* __restrict__ C, int accumulate) {
+    using T = float;
+    constexpr int VEC = 16 / sizeof(T);
+    constexpr int TC = kTiledStageBytes / (P * (int)sizeof(T));
+    constexpr int W = kTiledRowsPerWarp;
+    constexpr int R = kTiledRows;
+    constexpr int S = kTiledStages;
+    extern __shared__ __align__(128) unsigned char stages[];
+    __shared__ __align__(8) uint64_t full[S], empty[S];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int n_tiles = (n_cols + TC - 1) / TC;
+    const int64_t n_bands = (n_rows + R - 1) / R;
+    // bands blockIdx.x, blockIdx.x + gridDim.x, ...: one (band, tile) item after the other, the stages cycling
+    // through all of them, so the next band's first tiles load under the current band's last ones
+    const int64_t items = (n_bands - 1 - blockIdx.x) / gridDim.x * n_tiles + n_tiles;
+    auto issue = [&](int64_t i) {
+        const int lo = (int)(i % n_tiles) * TC;
+        const unsigned bytes = (unsigned)(min(TC, n_cols - lo) * P * (int)sizeof(T));
+        tma_load_1d(stages + (i % S) * kTiledStageBytes, B + (size_t)lo * P, bytes, &full[i % S]);
+    };
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < S; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], kTiledWarps);
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int64_t i = 0; i < S && i < items; ++i) issue(i);
+    }
+    __syncthreads();
+
+    float acc[W][VEC];
+    int c[W];        // window of row w: lane j holds entry rpos(w) + j
+    float v[W];
+    int64_t rstart = 0;  // lane w < W: first entry, length and consumed entries of row w
+    int rlen = 0, rpos = 0;
+    int64_t row0 = 0;
+    for (int64_t i = 0; i < items; ++i) {
+        const int tile = (int)(i % n_tiles);
+        if (tile == 0) {
+            row0 = (blockIdx.x + i / n_tiles * gridDim.x) * (int64_t)R + warp * W;
+            rstart = 0;
+            rlen = rpos = 0;
+            if (lane < W && row0 + lane < n_rows) {
+                rstart = __ldg(indptr + row0 + lane);
+                rlen = (int)(__ldg(indptr + row0 + lane + 1) - rstart);
+            }
+#pragma unroll
+            for (int w = 0; w < W; ++w) {
+#pragma unroll
+                for (int e = 0; e < VEC; ++e) acc[w][e] = 0.f;
+                load_window(indices, data, __shfl_sync(0xffffffffu, rstart, w), 0,
+                                   __shfl_sync(0xffffffffu, rlen, w), lane, c[w], v[w]);
+            }
+        }
+        const int s = (int)(i % S);
+        mbar_wait(&full[s], (unsigned)(i / S) & 1u);
+        const T* tl = reinterpret_cast<const T*>(stages + s * kTiledStageBytes);
+        const int lo = tile * TC, hi = min(lo + TC, n_cols);
+#pragma unroll
+        for (int w = 0; w < W; ++w) {
+            // sorted rows: the window's entries below hi are its first cnt lanes
+            int cnt = __popc(__ballot_sync(0xffffffffu, c[w] < hi));
+            if (cnt == 0) continue;
+            int pos = __shfl_sync(0xffffffffu, rpos, w);
+            const int64_t st = __shfl_sync(0xffffffffu, rstart, w);
+            const int len = __shfl_sync(0xffffffffu, rlen, w);
+            for (;;) {
+                gather_segment<P, T>(acc[w], tl, lo, c[w], v[w], pos, cnt, lane);
+                pos += cnt;
+                load_window(indices, data, st, pos, len, lane, c[w], v[w]);
+                if (cnt < 32) break;  // the reload is only needed at the next tile
+                cnt = __popc(__ballot_sync(0xffffffffu, c[w] < hi));
+                if (cnt == 0) break;
+            }
+            if (lane == w) rpos = pos;
+        }
+        // release the stage; warp 0 refills it with item i + S once all warps have
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+        if (threadIdx.x == 0 && i + S < items) {
+            mbar_wait(&empty[s], (unsigned)(i / S) & 1u);
+            issue(i + S);
+        }
+        __syncwarp();
+        if (tile == n_tiles - 1) {
+#pragma unroll
+            for (int w = 0; w < W; ++w)
+                if (row0 + w < n_rows) store_row<P, T>(acc[w], C + (size_t)(row0 + w) * P, accumulate, 1.f, lane);
+        }
+    }
+}
+
+template <int P>
+static int launch_spmm_tiled(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
+                             int n_cols, const float* B, float* C, int accumulate, cudaStream_t stream,
+                             const char* name) {
+    auto kernel = spmm_csr_tiled_kernel<P>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTiledSmemBytes);
+    MUB_REQUIRE(e == cudaSuccess, "%s: %s", name, cudaGetErrorString(e));
+    const int64_t bands = (n_rows + kTiledRows - 1) / kTiledRows;
+    // one CTA per SM, every CTA sweeping B at about the same pace: the tiles a CTA stages were just staged by the
+    // others and are still in L2
+    const int grid = (int)(bands < sm_count() ? bands : sm_count());
+    kernel<<<grid, kTiledThreads, kTiledSmemBytes, stream>>>(indptr, indices, data, n_rows, n_cols, B, C, accumulate);
+    return check_launch(name);
+}
+
+// the four C entry points: shared validation, then one instantiation per ld and schedule
 template <bool PAIRS, typename T>
 static int spmm_entry(const char* name, const int64_t* indptr, const int32_t* indices, const float* data,
                       int64_t n_rows, int64_t n_cols, const void* B, int32_t ld, float* C, int32_t accumulate,
-                      float out_scale, unsigned long long* row_counter, mub_stream_t stream) {
+                      float out_scale, unsigned long long* row_counter, uint32_t flags, mub_stream_t stream) {
     MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "%s: negative shape", name);
     MUB_REQUIRE(ld == 32 || ld == 64 || ld == 128, "%s: ld must be 32, 64 or 128 (got %d)", name, ld);
+    MUB_REQUIRE((flags & ~(uint32_t)MUB_SPMM_ROWS_SORTED) == 0, "%s: unknown flags 0x%x", name, flags);
     if (n_rows == 0) return 0;
     MUB_REQUIRE(indptr && B && C, "%s: null pointer", name);
     MUB_REQUIRE((((uintptr_t)B | (uintptr_t)C) & 15) == 0, "%s: B and C must be 16-byte aligned", name);
     MUB_REQUIRE(!PAIRS || ((uintptr_t)indices & 7) == 0, "%s: pairs must be 8-byte aligned", name);
     const T* Bt = (const T*)B;
     cudaStream_t s = (cudaStream_t)stream;
+    // measured on the LSI products (profiles/README.md): the tiled kernel wins on A*V with the fp32 operand.  With the
+    // half operand the row-warp kernel gathers half the bytes while the tiled kernel's cost per (row, tile) segment
+    // stays; on the pairs-layout A^T panels the operand slice already sits in L2 and the rows' skewed lengths want
+    // the row-warp kernel's dynamic scheduling
+    if constexpr (std::is_same_v<T, float> && !PAIRS) {
+        if ((flags & MUB_SPMM_ROWS_SORTED) && n_cols > 0) {
+            MUB_REQUIRE(n_cols < INT_MAX, "%s: n_cols must be below 2^31", name);
+            const int d = (int)n_cols;
+            switch (ld) {
+                case 32: return launch_spmm_tiled<32>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
+                case 64: return launch_spmm_tiled<64>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
+                default: return launch_spmm_tiled<128>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
+            }
+        }
+    }
     switch (ld) {
         case 32: return launch_spmm<32, PAIRS, T>(indptr, indices, data, n_rows, Bt, C, accumulate, out_scale, row_counter, s, name);
         case 64: return launch_spmm<64, PAIRS, T>(indptr, indices, data, n_rows, Bt, C, accumulate, out_scale, row_counter, s, name);
@@ -222,30 +441,32 @@ f32_to_f16_scaled_kernel(const float4* __restrict__ src, int64_t n4, float scale
 
 extern "C" int mub_spmm_csr_f32(const int64_t* indptr, const int32_t* indices, const float* data,
                                 int64_t n_rows, int64_t n_cols, const float* B, int32_t ld, float* C,
-                                int32_t accumulate, unsigned long long* row_counter, mub_stream_t stream) {
+                                int32_t accumulate, unsigned long long* row_counter, uint32_t flags,
+                                mub_stream_t stream) {
     return mub::spmm_entry<false, float>("spmm_csr", indptr, indices, data, n_rows, n_cols, B, ld, C, accumulate, 1.f,
-                                         row_counter, stream);
+                                         row_counter, flags, stream);
 }
 
 extern "C" int mub_spmm_csrp_f32(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, int64_t n_cols,
                                  const float* B, int32_t ld, float* C, int32_t accumulate,
-                                 unsigned long long* row_counter, mub_stream_t stream) {
+                                 unsigned long long* row_counter, uint32_t flags, mub_stream_t stream) {
     return mub::spmm_entry<true, float>("spmm_csrp", indptr, pairs, nullptr, n_rows, n_cols, B, ld, C, accumulate, 1.f,
-                                        row_counter, stream);
+                                        row_counter, flags, stream);
 }
 
 extern "C" int mub_spmm_csr_h16(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
                                 int64_t n_cols, const void* B_half, int32_t ld, float* C, int32_t accumulate,
-                                float out_scale, unsigned long long* row_counter, mub_stream_t stream) {
+                                float out_scale, unsigned long long* row_counter, uint32_t flags,
+                                mub_stream_t stream) {
     return mub::spmm_entry<false, __half>("spmm_csr_h16", indptr, indices, data, n_rows, n_cols, B_half, ld, C,
-                                          accumulate, out_scale, row_counter, stream);
+                                          accumulate, out_scale, row_counter, flags, stream);
 }
 
 extern "C" int mub_spmm_csrp_h16(const int64_t* indptr, const int32_t* pairs, int64_t n_rows, int64_t n_cols,
                                  const void* B_half, int32_t ld, float* C, int32_t accumulate, float out_scale,
-                                 unsigned long long* row_counter, mub_stream_t stream) {
+                                 unsigned long long* row_counter, uint32_t flags, mub_stream_t stream) {
     return mub::spmm_entry<true, __half>("spmm_csrp_h16", indptr, pairs, nullptr, n_rows, n_cols, B_half, ld, C,
-                                         accumulate, out_scale, row_counter, stream);
+                                         accumulate, out_scale, row_counter, flags, stream);
 }
 
 extern "C" int mub_f32_to_f16_scaled(const float* src, int64_t n, float scale, void* dst, mub_stream_t stream) {
