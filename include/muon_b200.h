@@ -334,6 +334,60 @@ int mub_synth_fill(int64_t row0, int64_t n_rows, int32_t n_cols, const float* be
                    const int32_t* row_topic, const float* row_scale, uint64_t seed, const int64_t* indptr,
                    int32_t* indices, float* data, mub_stream_t stream);
 
+/* ---- DSB normalisation of protein counts (muon/_prot/preproc.py:161-218) ------------------
+ * _f32 / _f64: the dtype of log(X + pseudocount), which is also the output dtype.  Count matrices
+ * are CSR (indptr != NULL; canonical: no duplicate entries) or dense row-major (indptr == NULL).
+ *   moments : mean[P] and ddof=1 stdev[P] (fp64) of log(x + pseudocount) over the empty droplets
+ *             (preproc.py:173-175); only stored entries are read.  Deterministic (fixed-order sums).
+ *   fit     : per cell, out[i,:] = (log(x + pc) - mean) [/ stdev if MUB_DSB_STANDARDIZE], rounded
+ *             to the output dtype (preproc.py:161-177); with MUB_DSB_FIT also the tied and full
+ *             2-component mixtures of preproc.py:183-198 in fp64 on the rounded row: bgmean[i] (min
+ *             mean of the model with the smaller BIC, full on a tie, rounded to the output dtype),
+ *             model[i] (0 tied, 1 full), n_iter[2i + m], converged[2i + m].  draws holds the uniform
+ *             P x 2 blocks of sklearn's init_params="random": the block of fit m of cell i starts at
+ *             draws + i*draw_cell_stride + m*draw_model_stride (strides 0: one block for every fit).
+ *             A row with a non-finite scaled value sets bit0 of *status (device int32, zeroed by the
+ *             caller) and gets bgmean NaN.
+ *   cross   : sums[q + q*q + P + q*P] = [sum z | sum z z^T | sum y_j | sum z y_j] over cells, with
+ *             z = [y[:, controls] | bgmean], q = n_controls + 1 <= MUB_DSB_MAX_CONTROLS + 1.
+ *   apply   : y[i,j] -= (z_i . w - b) * beta[j] (skipped when beta == NULL), then with MUB_DSB_CLIP
+ *             y[i,j] = min(max(y[i,j], lo), hi); arithmetic in fp64, rounded to the output dtype. */
+#define MUB_DSB_MAX_PROTEINS 1024
+#define MUB_DSB_MAX_CONTROLS 14
+#define MUB_DSB_STANDARDIZE 1u /* scale_factor="standardize" */
+#define MUB_DSB_FIT 2u         /* denoise_counts=True: run the mixture fits */
+#define MUB_DSB_CLIP 1u        /* quantile_clipping=True */
+size_t mub_dsb_moments_workspace_bytes(int64_t n_rows, int32_t n_prot);
+int mub_dsb_moments_f32(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
+                        int32_t n_prot, float pseudocount, void* workspace, double* mean, double* stdev,
+                        mub_stream_t stream);
+int mub_dsb_moments_f64(const int64_t* indptr, const int32_t* indices, const double* data, int64_t n_rows,
+                        int32_t n_prot, double pseudocount, void* workspace, double* mean, double* stdev,
+                        mub_stream_t stream);
+int mub_dsb_fit_f32(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_cells,
+                    int32_t n_prot, float pseudocount, const double* mean, const double* stdev, uint32_t flags,
+                    const double* draws, int64_t draw_cell_stride, int64_t draw_model_stride, float* out,
+                    double* bgmean, int8_t* model, int32_t* n_iter, int8_t* converged, int32_t* status,
+                    mub_stream_t stream);
+int mub_dsb_fit_f64(const int64_t* indptr, const int32_t* indices, const double* data, int64_t n_cells,
+                    int32_t n_prot, double pseudocount, const double* mean, const double* stdev, uint32_t flags,
+                    const double* draws, int64_t draw_cell_stride, int64_t draw_model_stride, double* out,
+                    double* bgmean, int8_t* model, int32_t* n_iter, int8_t* converged, int32_t* status,
+                    mub_stream_t stream);
+size_t mub_dsb_cross_workspace_bytes(int64_t n_cells, int32_t n_prot, int32_t n_controls);
+int mub_dsb_cross_f32(const float* y, int64_t n_cells, int32_t n_prot, const double* bgmean,
+                      const int32_t* controls, int32_t n_controls, void* workspace, double* sums,
+                      mub_stream_t stream);
+int mub_dsb_cross_f64(const double* y, int64_t n_cells, int32_t n_prot, const double* bgmean,
+                      const int32_t* controls, int32_t n_controls, void* workspace, double* sums,
+                      mub_stream_t stream);
+int mub_dsb_apply_f32(float* y, int64_t n_cells, int32_t n_prot, const double* bgmean, const int32_t* controls,
+                      int32_t n_controls, const double* w, double b, const double* beta, double lo, double hi,
+                      uint32_t flags, mub_stream_t stream);
+int mub_dsb_apply_f64(double* y, int64_t n_cells, int32_t n_prot, const double* bgmean, const int32_t* controls,
+                      int32_t n_controls, const double* w, double b, const double* beta, double lo, double hi,
+                      uint32_t flags, mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,11 +5,12 @@
     mu.atac.tl.lsi(adata)        # muon/_atac/tools.py:29
     mu.tl.mofa(mdata)            # muon/_core/tools.py:290
     mu.pp.neighbors(mdata)       # muon/_core/preproc.py:264  (WNN; first version, exact search)
+    mu.prot.pp.dsb(mdata, raw)   # muon/_prot/preproc.py:17   (DSB; per-cell mixture fits on the GPU)
 
 Same signatures and AnnData/MuData slot semantics as the reference; the arithmetic runs in
 hand-written CUDA kernels behind the C ABI in include/muon_b200.h.  There is no CPU fallback.
 """
-from . import atac, pp, tl  # noqa: F401
+from . import atac, pp, prot, tl  # noqa: F401
 from ._containers import SimpleAnnData, SimpleMuData  # noqa: F401
 from ._device import DeviceCSR, release_all_resident, release_resident, trim_host_cache  # noqa: F401
 

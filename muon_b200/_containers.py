@@ -227,6 +227,10 @@ class SimpleMuData:
     def __getitem__(self, key):
         if isinstance(key, str):
             return self.mod[key]
+        if isinstance(key, tuple):          # mdata[names, :] (muon/_prot/preproc.py:92)
+            key, cols = key
+            if not (isinstance(cols, slice) and cols == slice(None)):
+                raise NotImplementedError("SimpleMuData selects observations only: use mdata[names, :]")
         out = SimpleMuData({k: a[[n for n in key if n in set(a.obs_names)]] for k, a in self.mod.items()})
         return out
 

@@ -67,16 +67,28 @@ SIGNATURES = {
     "mub_device_fingerprint": [vp, i64, vp, vp],
     "mub_synth_count": [i64, i64, i32, vp, vp, vp, vp, u64, vp, vp],
     "mub_synth_fill": [i64, i64, i32, vp, vp, vp, vp, u64, vp, vp, vp, vp],
+    "mub_dsb_moments_f32": [vp, vp, vp, i64, i32, f32, vp, vp, vp, vp],
+    "mub_dsb_moments_f64": [vp, vp, vp, i64, i32, f64, vp, vp, vp, vp],
+    "mub_dsb_fit_f32": [vp, vp, vp, i64, i32, f32, vp, vp, u32, vp, i64, i64, vp, vp, vp, vp, vp, vp, vp],
+    "mub_dsb_fit_f64": [vp, vp, vp, i64, i32, f64, vp, vp, u32, vp, i64, i64, vp, vp, vp, vp, vp, vp, vp],
+    "mub_dsb_cross_f32": [vp, i64, i32, vp, vp, i32, vp, vp, vp],
+    "mub_dsb_cross_f64": [vp, i64, i32, vp, vp, i32, vp, vp, vp],
+    "mub_dsb_apply_f32": [vp, i64, i32, vp, vp, i32, vp, f64, vp, f64, f64, u32, vp],
+    "mub_dsb_apply_f64": [vp, i64, i32, vp, vp, i32, vp, f64, vp, f64, f64, u32, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
     "mub_gram_workspace_bytes": ([i64, i32], C.c_size_t),
     "mub_wnn_bandwidth_workspace_bytes": ([i32, i32], C.c_size_t),
     "mub_knn_l2_tc_workspace_bytes": ([i64, i64, i32], C.c_size_t),
+    "mub_dsb_moments_workspace_bytes": ([i64, i32], C.c_size_t),
+    "mub_dsb_cross_workspace_bytes": ([i64, i32, i32], C.c_size_t),
 }
 
 TFIDF_LOG_TF, TFIDF_LOG_IDF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE, TFIDF_BINARIZE = 1, 2, 4, 8, 16
 SPMM_ROWS_SORTED = 1
+DSB_STANDARDIZE, DSB_FIT, DSB_CLIP = 1, 2, 1
+DSB_MAX_PROTEINS, DSB_MAX_CONTROLS = 1024, 14
 
 
 class MuonB200Error(RuntimeError):
@@ -111,7 +123,8 @@ def load():
 
 # kernels launched per successful call (for the benchmark's gpu_launches claim)
 KERNELS_PER_CALL = {"mub_csr_transpose_fill_tiled": 2, "mub_csr_transpose_fill": 2, "mub_csr_transpose_fill_pairs": 2, "mub_gram_f32": 2, "mub_version": 0, "mub_device_info": 0,
-                    "mub_tfidf_tile_rows": 0, "mub_stager_create": 0, "mub_stager_destroy": 0, "mub_stager_h2d": 0, "mub_stager_d2h": 0, "mub_host_fingerprint": 0}
+                    "mub_tfidf_tile_rows": 0, "mub_stager_create": 0, "mub_stager_destroy": 0, "mub_stager_h2d": 0, "mub_stager_d2h": 0, "mub_host_fingerprint": 0,
+                    "mub_dsb_moments_f32": 4, "mub_dsb_moments_f64": 4, "mub_dsb_cross_f32": 2, "mub_dsb_cross_f64": 2}
 LAUNCHES = 0          # running count of kernels launched through this binding
 PROFILE = None        # None, or dict name -> list[(start_event, end_event)] filled by call()
 

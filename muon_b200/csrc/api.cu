@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 100; /* 0.1.0 */ }
+int mub_version(void) { return 101; /* 0.1.1: DSB */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 
