@@ -388,6 +388,24 @@ int mub_dsb_apply_f64(double* y, int64_t n_cells, int32_t n_prot, const double* 
                       int32_t n_controls, const double* w, double b, const double* beta, double lo, double hi,
                       uint32_t flags, mub_stream_t stream);
 
+/* ---- UMAP layout (umap-learn optimize_layout_euclidean, as scanpy's sc.tl.umap calls it) ------------------
+ *   epoch  : one Jacobi epoch.  Reads Y_in [n x dim] and writes Y_out (must not alias).  The head entries are the
+ *            CSR (indptr, indices) of the pruned graph, the tail entries its transpose (t_indptr, t_indices); eps /
+ *            t_eps hold each entry's epochs per sample w_max / w >= 1.  Entry e is sampled at epoch n iff
+ *            floor(n/eps) > floor((n-1)/eps); its m-th sample draws floor(n*rate/eps) - floor(n'*rate/eps)
+ *            negatives (n' = ceil((m-1)*eps), the first sample counts from 1 instead), vertex
+ *            philox4x32_10(ctr = {e_lo, e_hi ^ s2, n, draw}, key = {s0, s1}).x mod n.  Y_out[i] = Y_in[i] +
+ *            alpha_n * (sum of the clipped attraction terms of the sampled head and tail entries of i and the
+ *            repulsion terms of their negatives, skipping draws equal to i).  Deterministic: fixed-order sums.
+ *   philox : out[4t..4t+3] = Philox4x32-10(ctr[4t..4t+3], {k0, k1}) for t < n (the generator of the epoch). */
+#define MUB_UMAP_MAX_COMPONENTS 16
+int mub_umap_epoch_f32(const int64_t* indptr, const int32_t* indices, const float* eps, const int64_t* t_indptr,
+                       const int32_t* t_indices, const float* t_eps, int64_t n, int32_t dim, const float* Y_in,
+                       float* Y_out, float a, float b, float gamma, float alpha_n, int32_t epoch,
+                       int32_t negative_sample_rate, uint32_t s0, uint32_t s1, uint32_t s2, mub_stream_t stream);
+int mub_philox4x32_10(const uint32_t* ctr, int64_t n, uint32_t k0, uint32_t k1, uint32_t* out,
+                      mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,6 +6,7 @@
     mu.tl.mofa(mdata)            # muon/_core/tools.py:290
     mu.pp.neighbors(mdata)       # muon/_core/preproc.py:264  (WNN; first version, exact search)
     mu.prot.pp.dsb(mdata, raw)   # muon/_prot/preproc.py:17   (DSB; per-cell mixture fits on the GPU)
+    mu.tl.umap(mdata)            # muon/_core/tools.py:1209  (UMAP layout; Jacobi SGD epochs on the GPU)
 
 Same signatures and AnnData/MuData slot semantics as the reference; the arithmetic runs in
 hand-written CUDA kernels behind the C ABI in include/muon_b200.h.  There is no CPU fallback.

@@ -75,6 +75,8 @@ SIGNATURES = {
     "mub_dsb_cross_f64": [vp, i64, i32, vp, vp, i32, vp, vp, vp],
     "mub_dsb_apply_f32": [vp, i64, i32, vp, vp, i32, vp, f64, vp, f64, f64, u32, vp],
     "mub_dsb_apply_f64": [vp, i64, i32, vp, vp, i32, vp, f64, vp, f64, f64, u32, vp],
+    "mub_umap_epoch_f32": [vp, vp, vp, vp, vp, vp, i64, i32, vp, vp, f32, f32, f32, f32, i32, i32, u32, u32, u32, vp],
+    "mub_philox4x32_10": [vp, i64, u32, u32, vp, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
@@ -89,6 +91,7 @@ TFIDF_LOG_TF, TFIDF_LOG_IDF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE, TFIDF_BINARIZE = 1
 SPMM_ROWS_SORTED = 1
 DSB_STANDARDIZE, DSB_FIT, DSB_CLIP = 1, 2, 1
 DSB_MAX_PROTEINS, DSB_MAX_CONTROLS = 1024, 14
+UMAP_MAX_COMPONENTS = 16
 
 
 class MuonB200Error(RuntimeError):

@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 101; /* 0.1.1: DSB */ }
+int mub_version(void) { return 102; /* 0.1.2: UMAP layout */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 

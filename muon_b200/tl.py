@@ -1,4 +1,4 @@
-"""``mu.tl`` -- multimodal tools.  ``mofa`` is on the hot path (SURVEY section 8, rows a9-a11)."""
+"""``mu.tl`` -- multimodal tools.  ``mofa`` (SURVEY section 8, rows a9-a11) and ``umap`` run on the GPU."""
 from __future__ import annotations
 
 
@@ -6,3 +6,9 @@ def mofa(data, *args, **kwargs):
     """Multi-Omics Factor Analysis -- drop-in for ``muon.tl.mofa`` (muon/_core/tools.py:290-708)."""
     from ._mofa import mofa as _impl
     return _impl(data, *args, **kwargs)
+
+
+def umap(mdata, *args, **kwargs):
+    """UMAP layout of the neighbour graph on the GPU -- drop-in for ``muon.tl.umap`` (muon/_core/tools.py:1209-1362)."""
+    from ._umap import umap as _impl
+    return _impl(mdata, *args, **kwargs)
