@@ -406,6 +406,40 @@ int mub_umap_epoch_f32(const int64_t* indptr, const int32_t* indices, const floa
 int mub_philox4x32_10(const uint32_t* ctr, int64_t n, uint32_t k0, uint32_t k1, uint32_t* out,
                       mub_stream_t stream);
 
+/* ---- Leiden / Louvain (leidenalg / louvain-igraph on the multiplex RB-configuration objective) --------------------
+ * One graph per level: CSR (indptr, indices) with int64 fixed-point weights w (sum_l w_l A^l_uv * 2^Se) and degrees
+ * k [n x n_layers] (k^l_v * 2^Sk); ce = 2^-Se, cl_h[l] = w_l gamma_l / m_l * 2^-2Sk.  All sums are exact integer sums.
+ * Every pointer is device memory except cl_h, a host array of n_layers doubles read at launch.
+ *   scan    : mode 0 (local moving): for every vertex the best move out of memb[v] (neighbour communities, or the
+ *             empty community n + v), target[v] = -1 unless its gain exceeds 2^-40 of its magnitude.  mode 1
+ *             (refinement): memb is the refined partition, parent the communities; singletons whose coin for `key`
+ *             is set move to the best sub-community of their parent they touch (gain >= 0) that is not a moving
+ *             singleton; flags bit 0 is set when some singleton still has a non-negative move.  K / size are the
+ *             totals of memb.  Rows longer than mub_leiden_max_shared_degree() go through hubs[n_hubs] with a table
+ *             of hub_slots[i] (a power of two >= 2 x degree) slots at hub_off[i] in hub_keys / hub_vals (int64), and
+ *             hub_slots[i] / 2 list entries at hub_off[i] / 2 in hub_lists.
+ *   apply   : mode 0: prio[v] = the unique hashed priority of v's proposal (0 without one, prio is [n] uint64) and the
+ *             proposals with priority >= min_priority move; mode 1: every proposal moves (prio unused).  counts =
+ *             {moves, moves to an empty community}.
+ *   totals  : K[c] = sum of k over memb == c, size[c] = members (size may be NULL).
+ *   segment_sum : out[seg[i]] += w[i].   internal : out = sum of w over the entries inside one community. */
+#define MUB_LEIDEN_MAX_LAYERS 4
+int mub_leiden_scan(int32_t mode, const int64_t* indptr, const int32_t* indices, const int64_t* w, const int64_t* k,
+                    int64_t n, int32_t n_layers, double ce, const double* cl_h, const int32_t* memb,
+                    const int32_t* parent, const int64_t* K, const int32_t* size, uint64_t key, int32_t* target,
+                    double* gain, int32_t* flags, const int32_t* hubs, int64_t n_hubs, const int64_t* hub_off,
+                    const int32_t* hub_slots, int32_t* hub_keys, void* hub_vals, int32_t* hub_lists,
+                    int32_t* hub_counts, mub_stream_t stream);
+int32_t mub_leiden_max_shared_degree(void);
+int mub_leiden_apply(int32_t mode, int64_t n, int32_t* memb, const int32_t* target, uint64_t key,
+                     uint64_t min_priority, void* prio, int32_t* counts, mub_stream_t stream);
+int mub_leiden_totals(int64_t n, int32_t n_layers, const int32_t* memb, const int64_t* k, int64_t n_comm, int64_t* K,
+                      int32_t* size, mub_stream_t stream);
+int mub_leiden_segment_sum(int64_t n, const int64_t* seg, const int64_t* w, int64_t n_seg, int64_t* out,
+                           mub_stream_t stream);
+int mub_leiden_internal(int64_t n, const int64_t* indptr, const int32_t* indices, const int64_t* w,
+                        const int32_t* memb, int64_t* out, mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -77,6 +77,13 @@ SIGNATURES = {
     "mub_dsb_apply_f64": [vp, i64, i32, vp, vp, i32, vp, f64, vp, f64, f64, u32, vp],
     "mub_umap_epoch_f32": [vp, vp, vp, vp, vp, vp, i64, i32, vp, vp, f32, f32, f32, f32, i32, i32, u32, u32, u32, vp],
     "mub_philox4x32_10": [vp, i64, u32, u32, vp, vp],
+    "mub_leiden_scan": [i32, vp, vp, vp, vp, i64, i32, f64, vp, vp, vp, vp, vp, u64, vp, vp, vp, vp, i64, vp, vp, vp,
+                        vp, vp, vp, vp],
+    "mub_leiden_max_shared_degree": [],
+    "mub_leiden_apply": [i32, i64, vp, vp, u64, u64, vp, vp, vp],
+    "mub_leiden_totals": [i64, i32, vp, vp, i64, vp, vp, vp],
+    "mub_leiden_segment_sum": [i64, vp, vp, i64, vp, vp],
+    "mub_leiden_internal": [i64, vp, vp, vp, vp, vp, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
@@ -92,6 +99,7 @@ SPMM_ROWS_SORTED = 1
 DSB_STANDARDIZE, DSB_FIT, DSB_CLIP = 1, 2, 1
 DSB_MAX_PROTEINS, DSB_MAX_CONTROLS = 1024, 14
 UMAP_MAX_COMPONENTS = 16
+LEIDEN_MAX_LAYERS = 4
 
 
 class MuonB200Error(RuntimeError):
@@ -127,7 +135,8 @@ def load():
 # kernels launched per successful call (for the benchmark's gpu_launches claim)
 KERNELS_PER_CALL = {"mub_csr_transpose_fill_tiled": 2, "mub_csr_transpose_fill": 2, "mub_csr_transpose_fill_pairs": 2, "mub_gram_f32": 2, "mub_version": 0, "mub_device_info": 0,
                     "mub_tfidf_tile_rows": 0, "mub_stager_create": 0, "mub_stager_destroy": 0, "mub_stager_h2d": 0, "mub_stager_d2h": 0, "mub_host_fingerprint": 0,
-                    "mub_dsb_moments_f32": 4, "mub_dsb_moments_f64": 4, "mub_dsb_cross_f32": 2, "mub_dsb_cross_f64": 2}
+                    "mub_dsb_moments_f32": 4, "mub_dsb_moments_f64": 4, "mub_dsb_cross_f32": 2, "mub_dsb_cross_f64": 2,
+                    "mub_leiden_max_shared_degree": 0}
 LAUNCHES = 0          # running count of kernels launched through this binding
 PROFILE = None        # None, or dict name -> list[(start_event, end_event)] filled by call()
 

@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 102; /* 0.1.2: UMAP layout */ }
+int mub_version(void) { return 103; /* 0.1.3: Leiden / Louvain */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 

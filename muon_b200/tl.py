@@ -12,3 +12,15 @@ def umap(mdata, *args, **kwargs):
     """UMAP layout of the neighbour graph on the GPU -- drop-in for ``muon.tl.umap`` (muon/_core/tools.py:1209-1362)."""
     from ._umap import umap as _impl
     return _impl(mdata, *args, **kwargs)
+
+
+def leiden(data, *args, **kwargs):
+    """Multiplex Leiden clustering on the GPU -- drop-in for ``muon.tl.leiden`` (muon/_core/tools.py:1057)."""
+    from ._leiden import leiden as _impl
+    return _impl(data, *args, **kwargs)
+
+
+def louvain(data, *args, **kwargs):
+    """Multiplex Louvain clustering on the GPU -- drop-in for ``muon.tl.louvain`` (muon/_core/tools.py:1133)."""
+    from ._leiden import louvain as _impl
+    return _impl(data, *args, **kwargs)
