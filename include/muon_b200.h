@@ -119,6 +119,11 @@ int mub_csr_transpose_fill(const int64_t* indptr, const int32_t* indices, const 
                            int64_t n_rows, int32_t n_cols, int64_t row_offset,
                            const int64_t* t_indptr, int64_t* cursor, int32_t* t_indices,
                            float* t_data, mub_stream_t stream);
+/* the same fill for float64 values (differential accessibility ranks a float64 matrix on its own values) */
+int mub_csr_transpose_fill_f64(const int64_t* indptr, const int32_t* indices, const double* data,
+                               int64_t n_rows, int32_t n_cols, int64_t row_offset,
+                               const int64_t* t_indptr, int64_t* cursor, int32_t* t_indices,
+                               double* t_data, mub_stream_t stream);
 
 /* "Pairs" layout for transposed panels: entry k of row j is the 8-byte pair {int32 index, float32 value bits},
  * so the scatter writes once per non-zero and the product reads one 8-byte word per entry.
@@ -439,6 +444,42 @@ int mub_leiden_segment_sum(int64_t n, const int64_t* seg, const int64_t* w, int6
                            mub_stream_t stream);
 int mub_leiden_internal(int64_t n, const int64_t* indptr, const int32_t* indices, const int64_t* w,
                         const int32_t* memb, int64_t* out, mub_stream_t stream);
+
+/* ---- differential accessibility (scanpy's rank_genes_groups, called by muon/_atac/tools.py:371) ------------------
+ * Input: the CSR of A^T (t_indptr [d+1], t_cells [nnz], t_vals [nnz]) and cell_code [n cells]: 0..K-2 = the tested
+ * groups, K-1 = the other ranked cells (rest: cells of no tested group; MUB_RANK_VS_GROUP: the reference group),
+ * -1 = not ranked (MUB_RANK_VS_GROUP only).  group_n [K] = cells per code; n_ranked = cells with a code >= 0
+ * (< 2642245, so that the tie terms are exact in 64 bits).  K - 1 <= MUB_RANK_MAX_GROUPS.
+ *   stats : rows [n_rows] of A^T, written to columns cols [n_rows] of stats [5][K][n_out] (float64): stored non-zeros,
+ *           sum, sum of squares (each value squared in the input precision), rank sum, tie term sum(t^3 - t).  Rank sum
+ *           (codes < K-1, MUB_RANK_WILCOXON): the group's average ranks among all ranked cells (rest), or among the
+ *           group and the reference (MUB_RANK_VS_GROUP); exact.  The tie term is that of the same ranking.  Stored
+ *           zeros count as implicit zeros; negative values rank below them.  Moments are fixed-order sums: the output
+ *           does not depend on the entry order of the transposition.  cap: a power of two >= every row's length; rows
+ *           up to mub_rank_shared_capacity() are sorted in shared memory (cap = the size class), longer ones in a
+ *           workspace of ws_bytes >= mub_rank_workspace_slice_bytes(cap) (one slice per concurrently sorted row).
+ *   score : per (group g < K-1, column) from stats: scores / pvals (Welch's t and its two-sided p, or the Wilcoxon z
+ *           and erfc(|z|/sqrt 2); NaN score -> 0, NaN p -> 1), lfc = log2((expm1(mean_g) + 1e-9) / (expm1(mean_r) +
+ *           1e-9)) (expm1(x ln base) when log_base > 0), pts [K][n_out] = stored non-zeros / cells (row K-1 with
+ *           MUB_RANK_VS_GROUP only), pts_rest [K-1][n_out] (rest only, may be NULL).  n_total = cells of the matrix. */
+#define MUB_RANK_WILCOXON 1u
+#define MUB_RANK_VS_GROUP 2u
+#define MUB_RANK_TIE_CORRECT 4u
+#define MUB_RANK_OVERESTIM_VAR 8u
+#define MUB_RANK_MAX_GROUPS 1024
+int32_t mub_rank_shared_capacity(int32_t value_bytes);
+int64_t mub_rank_workspace_slice_bytes(int32_t value_bytes, int32_t cap);
+int mub_rank_stats_f32(const int64_t* t_indptr, const int32_t* t_cells, const float* t_vals, const int32_t* cell_code,
+                       const int32_t* rows, const int32_t* cols, int32_t n_rows, int32_t n_out, int32_t K,
+                       const int64_t* group_n, int64_t n_ranked, uint32_t flags, int32_t cap, void* ws, int64_t ws_bytes,
+                       double* stats, mub_stream_t stream);
+int mub_rank_stats_f64(const int64_t* t_indptr, const int32_t* t_cells, const double* t_vals, const int32_t* cell_code,
+                       const int32_t* rows, const int32_t* cols, int32_t n_rows, int32_t n_out, int32_t K,
+                       const int64_t* group_n, int64_t n_ranked, uint32_t flags, int32_t cap, void* ws, int64_t ws_bytes,
+                       double* stats, mub_stream_t stream);
+int mub_rank_score(const double* stats, int32_t K, int32_t n_out, const int64_t* group_n, int64_t n_total,
+                   uint32_t flags, double log_base, double* scores, double* pvals, double* lfc, double* pts,
+                   double* pts_rest, mub_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -7,6 +7,7 @@
     mu.pp.neighbors(mdata)       # muon/_core/preproc.py:264  (WNN; first version, exact search)
     mu.prot.pp.dsb(mdata, raw)   # muon/_prot/preproc.py:17   (DSB; per-cell mixture fits on the GPU)
     mu.tl.umap(mdata)            # muon/_core/tools.py:1209  (UMAP layout; Jacobi SGD epochs on the GPU)
+    mu.atac.tl.rank_peaks_groups(atac, "leiden")   # muon/_atac/tools.py:337  (t-test / Wilcoxon per peak on the GPU)
 
 Same signatures and AnnData/MuData slot semantics as the reference; the arithmetic runs in
 hand-written CUDA kernels behind the C ABI in include/muon_b200.h.  There is no CPU fallback.

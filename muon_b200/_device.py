@@ -615,15 +615,15 @@ def csr_transpose(A: DeviceCSR) -> DeviceCSR:
     """The CSR of A^T on the device (count -> scan -> atomic-cursor fill).  The order of the entries inside a transposed
     row follows the fill's slot claims."""
     require_cuda()
-    assert A.data.dtype == torch.float32, "transpose: float32 values only"
+    assert A.data.dtype in (torch.float32, torch.float64), "transpose: float32 or float64 values only"
     n, d = A.shape
     dev = A.data.device
     t_indptr = _transposed_indptr(A, 0, A.nnz, None)
     cursor = torch.empty(max(d, 1), dtype=torch.int64, device=dev)
     t_indices = torch.empty(A.nnz, dtype=torch.int32, device=dev)
-    t_data = torch.empty(A.nnz, dtype=torch.float32, device=dev)
-    call("mub_csr_transpose_fill", ptr(A.indptr), ptr(A.indices), ptr(A.data), n, d, 0, ptr(t_indptr), ptr(cursor),
-         ptr(t_indices), ptr(t_data), stream_ptr())
+    t_data = torch.empty(A.nnz, dtype=A.data.dtype, device=dev)
+    call("mub_csr_transpose_fill_f64" if A.data.dtype == torch.float64 else "mub_csr_transpose_fill", ptr(A.indptr),
+         ptr(A.indices), ptr(A.data), n, d, 0, ptr(t_indptr), ptr(cursor), ptr(t_indices), ptr(t_data), stream_ptr())
     return DeviceCSR(t_indptr, t_indices, t_data, (d, n), n_total=d, sorted_indices=False)
 
 

@@ -36,6 +36,7 @@ SIGNATURES = {
     "mub_spmm_csr_f32": [vp, vp, vp, i64, i64, vp, i32, vp, i32, vp, u32, vp],
     "mub_csr_transpose_count": [vp, i64, i32, vp, vp],
     "mub_csr_transpose_fill": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp, vp],
+    "mub_csr_transpose_fill_f64": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp, vp],
     "mub_gram_f32": [vp, vp, i64, i32, i32, vp, vp, vp],
     "mub_csr_transpose_fill_pairs": [vp, vp, vp, i64, i32, i64, vp, vp, vp, vp],
     "mub_spmm_csrp_f32": [vp, vp, i64, i64, vp, i32, vp, i32, vp, u32, vp],
@@ -84,6 +85,9 @@ SIGNATURES = {
     "mub_leiden_totals": [i64, i32, vp, vp, i64, vp, vp, vp],
     "mub_leiden_segment_sum": [i64, vp, vp, i64, vp, vp],
     "mub_leiden_internal": [i64, vp, vp, vp, vp, vp, vp],
+    "mub_rank_stats_f32": [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, i64, u32, i32, vp, i64, vp, vp],
+    "mub_rank_stats_f64": [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, i64, u32, i32, vp, i64, vp, vp],
+    "mub_rank_score": [vp, i32, i32, vp, i64, u32, f64, vp, vp, vp, vp, vp, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
@@ -92,6 +96,8 @@ SPECIAL_RESTYPE = {
     "mub_knn_l2_tc_workspace_bytes": ([i64, i64, i32], C.c_size_t),
     "mub_dsb_moments_workspace_bytes": ([i64, i32], C.c_size_t),
     "mub_dsb_cross_workspace_bytes": ([i64, i32, i32], C.c_size_t),
+    "mub_rank_shared_capacity": ([i32], i32),
+    "mub_rank_workspace_slice_bytes": ([i32, i32], i64),
 }
 
 TFIDF_LOG_TF, TFIDF_LOG_IDF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE, TFIDF_BINARIZE = 1, 2, 4, 8, 16
@@ -100,6 +106,8 @@ DSB_STANDARDIZE, DSB_FIT, DSB_CLIP = 1, 2, 1
 DSB_MAX_PROTEINS, DSB_MAX_CONTROLS = 1024, 14
 UMAP_MAX_COMPONENTS = 16
 LEIDEN_MAX_LAYERS = 4
+RANK_WILCOXON, RANK_VS_GROUP, RANK_TIE_CORRECT, RANK_OVERESTIM_VAR = 1, 2, 4, 8
+RANK_MAX_GROUPS = 1024
 
 
 class MuonB200Error(RuntimeError):
@@ -133,7 +141,7 @@ def load():
 
 
 # kernels launched per successful call (for the benchmark's gpu_launches claim)
-KERNELS_PER_CALL = {"mub_csr_transpose_fill_tiled": 2, "mub_csr_transpose_fill": 2, "mub_csr_transpose_fill_pairs": 2, "mub_gram_f32": 2, "mub_version": 0, "mub_device_info": 0,
+KERNELS_PER_CALL = {"mub_csr_transpose_fill_tiled": 2, "mub_csr_transpose_fill": 2, "mub_csr_transpose_fill_f64": 2, "mub_csr_transpose_fill_pairs": 2, "mub_gram_f32": 2, "mub_version": 0, "mub_device_info": 0,
                     "mub_tfidf_tile_rows": 0, "mub_stager_create": 0, "mub_stager_destroy": 0, "mub_stager_h2d": 0, "mub_stager_d2h": 0, "mub_host_fingerprint": 0,
                     "mub_dsb_moments_f32": 4, "mub_dsb_moments_f64": 4, "mub_dsb_cross_f32": 2, "mub_dsb_cross_f64": 2,
                     "mub_leiden_max_shared_degree": 0}

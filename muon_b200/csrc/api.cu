@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 103; /* 0.1.3: Leiden / Louvain */ }
+int mub_version(void) { return 104; /* 0.1.4: differential accessibility (rank_peaks_groups) */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 

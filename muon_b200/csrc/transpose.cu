@@ -39,10 +39,11 @@ __global__ void copy_i64_kernel(const int64_t* __restrict__ src, int64_t* __rest
 // PAIRS: (row, value) is written as ONE 8-byte pair (int2, in t_indices; t_data unused) instead of into two arrays:
 // one scattered store per non-zero instead of two (the fill is bound by the rate of scattered L2 operations, not by
 // bytes).
-template <bool PAIRS>
-__device__ __forceinline__ void store_entry(int32_t* __restrict__ t_indices, float* __restrict__ t_data,
-                                            unsigned long long slot, int32_t r, float v) {
+template <bool PAIRS, typename V>
+__device__ __forceinline__ void store_entry(int32_t* __restrict__ t_indices, V* __restrict__ t_data,
+                                            unsigned long long slot, int32_t r, V v) {
     if constexpr (PAIRS) {
+        static_assert(sizeof(V) == 4, "pairs hold float32 values");
         reinterpret_cast<int2*>(t_indices)[slot] = make_int2(r, __float_as_int(v));
     } else {
         t_indices[slot] = r;
@@ -50,11 +51,11 @@ __device__ __forceinline__ void store_entry(int32_t* __restrict__ t_indices, flo
     }
 }
 
-template <bool PAIRS>
+template <bool PAIRS, typename V>
 __global__ void __launch_bounds__(256)
 transpose_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                      const float* __restrict__ data, int64_t n_rows, int64_t row_offset,
-                      unsigned long long* cursor, int32_t* __restrict__ t_indices, float* __restrict__ t_data) {
+                      const V* __restrict__ data, int64_t n_rows, int64_t row_offset,
+                      unsigned long long* cursor, int32_t* __restrict__ t_indices, V* __restrict__ t_data) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int64_t n_warps = (int64_t)gridDim.x * 8;
@@ -66,8 +67,8 @@ transpose_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
         for (; k + 96 < e; k += 128) {
             const int c0 = ld_stream(indices + k), c1 = ld_stream(indices + k + 32);
             const int c2 = ld_stream(indices + k + 64), c3 = ld_stream(indices + k + 96);
-            const float v0 = ld_stream(data + k), v1 = ld_stream(data + k + 32);
-            const float v2 = ld_stream(data + k + 64), v3 = ld_stream(data + k + 96);
+            const V v0 = ld_stream(data + k), v1 = ld_stream(data + k + 32);
+            const V v2 = ld_stream(data + k + 64), v3 = ld_stream(data + k + 96);
             const unsigned long long s0 = atomicAdd(cursor + c0, 1ull), s1 = atomicAdd(cursor + c1, 1ull);
             const unsigned long long s2 = atomicAdd(cursor + c2, 1ull), s3 = atomicAdd(cursor + c3, 1ull);
             store_entry<PAIRS>(t_indices, t_data, s0, r, v0);
@@ -77,17 +78,17 @@ transpose_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
         }
         for (; k < e; k += 32) {
             const int c = ld_stream(indices + k);
-            const float v = ld_stream(data + k);
+            const V v = ld_stream(data + k);
             store_entry<PAIRS>(t_indices, t_data, atomicAdd(cursor + c, 1ull), r, v);
         }
     }
 }
 
 // the two atomic-cursor entry points: shared validation, cursors seeded from the scanned histogram, one warp per row
-template <bool PAIRS>
-static int launch_transpose_fill(const char* name, const int64_t* indptr, const int32_t* indices, const float* data,
+template <bool PAIRS, typename V>
+static int launch_transpose_fill(const char* name, const int64_t* indptr, const int32_t* indices, const V* data,
                                  int64_t n_rows, int32_t n_cols, int64_t row_offset, const int64_t* t_indptr,
-                                 int64_t* cursor, int32_t* t_indices, float* t_data, mub_stream_t stream) {
+                                 int64_t* cursor, int32_t* t_indices, V* t_data, mub_stream_t stream) {
     MUB_REQUIRE(n_rows >= 0 && n_cols >= 0, "%s: negative shape", name);
     if (n_rows == 0 || n_cols == 0) return 0;
     MUB_REQUIRE(indptr && t_indptr && cursor && t_indices && (PAIRS || t_data), "%s: null pointer", name);
@@ -98,7 +99,7 @@ static int launch_transpose_fill(const char* name, const int64_t* indptr, const 
     int64_t cap = (int64_t)sm_count() * 8;
     int grid = (int)(want < cap ? want : cap);
     if (grid < 1) grid = 1;
-    transpose_fill_kernel<PAIRS><<<grid, 256, 0, s>>>(indptr, indices, data, n_rows, row_offset,
+    transpose_fill_kernel<PAIRS, V><<<grid, 256, 0, s>>>(indptr, indices, data, n_rows, row_offset,
                                                      (unsigned long long*)cursor, t_indices, t_data);
     return check_launch(name);
 }
@@ -367,7 +368,7 @@ extern "C" {
 int mub_csr_transpose_fill_pairs(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
                                  int32_t n_cols, int64_t row_offset, const int64_t* t_indptr, int64_t* cursor,
                                  int32_t* t_pairs, mub_stream_t stream) {
-    return mub::launch_transpose_fill<true>("transpose_fill_pairs", indptr, indices, data, n_rows, n_cols, row_offset,
+    return mub::launch_transpose_fill<true, float>("transpose_fill_pairs", indptr, indices, data, n_rows, n_cols, row_offset,
                                             t_indptr, cursor, t_pairs, nullptr, stream);
 }
 
@@ -404,6 +405,13 @@ int mub_csr_transpose_fill(const int64_t* indptr, const int32_t* indices, const 
                            int32_t n_cols, int64_t row_offset, const int64_t* t_indptr, int64_t* cursor,
                            int32_t* t_indices, float* t_data, mub_stream_t stream) {
     return mub::launch_transpose_fill<false>("transpose_fill", indptr, indices, data, n_rows, n_cols, row_offset,
+                                             t_indptr, cursor, t_indices, t_data, stream);
+}
+
+int mub_csr_transpose_fill_f64(const int64_t* indptr, const int32_t* indices, const double* data, int64_t n_rows,
+                               int32_t n_cols, int64_t row_offset, const int64_t* t_indptr, int64_t* cursor,
+                               int32_t* t_indices, double* t_data, mub_stream_t stream) {
+    return mub::launch_transpose_fill<false>("transpose_fill_f64", indptr, indices, data, n_rows, n_cols, row_offset,
                                              t_indptr, cursor, t_indices, t_data, stream);
 }
 
