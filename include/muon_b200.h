@@ -481,6 +481,52 @@ int mub_rank_score(const double* stats, int32_t K, int32_t n_out, const int64_t*
                    uint32_t flags, double log_base, double* scores, double* pvals, double* lfc, double* pts,
                    double* pts_rest, mub_stream_t stream);
 
+/* ---- fragments file (muon/_atac/tools.py:746-1201: count_fragments_features, tss_enrichment, nucleosome_signal) ------
+ * text: an inflated chunk of the fragments file whose last byte is a newline.
+ *   newline_count / newline_fill : tile_counts [ceil(n_bytes / mub_frag_tile_bytes())] newlines per tile; with their
+ *           exclusive scan tile_offsets, nl_pos [lines] receives every newline position in byte order.
+ *   barcode_table : open addressing over the barcodes bc[bc_off[j] : bc_off[j+1]] (distinct, j < n_bc): keys [capacity]
+ *           (zeroed; a power of two > n_bc) hold 64-bit hashes, slot_entry [capacity] the barcode index j.
+ *   parse : one thread per line: start, end (int32), score (int32) of the 5 tab-separated fields, cell = bc_val[j] of the
+ *           barcode equal byte for byte to the name field, else -1 (keys may be NULL: no lookup).  flags: bit0 = the
+ *           line starts a contig run (first line, or a chromosome unlike the previous line's), bit1 = a '#' line.
+ *           status int64[5] (caller initialises {INT64_MAX x3, 0, 0}): atomic minimum line_base + line of a malformed
+ *           line, of a coordinate or score beyond int32, of a start below the previous line's on the same chromosome;
+ *           maximum fragment length; count of '#' lines.
+ *   overlap : one warp per query q over records [q_rec_lo, q_rec_hi) (one contig, start-sorted): hits are records with
+ *           start < q_hi, end > q_lo and cell >= 0, searched from the first start >= q_lo - lmax + 1.  out_off NULL:
+ *           counts [n_q] = hits; else hits go to out_off[q].. in record order as (cell, feat_base + q, score or 1).
+ *   tss_pileup : same hits; +score at max(start - q_lo, 0) and -score at min(end - q_lo, width) of the cell's row of
+ *           diff [cells][width + 1] (int64, zeroed).
+ *   tss_rows : per cell, diff row -> its running sum (the pileup, in place); sums [cells][2] = sum over the first and the
+ *           last `flank` positions, sum over [center_lo, center_hi).
+ *   tss_scale : out [cells][width] = pile / flank_mean[cell] (float64, IEEE division).
+ *   nucleosome : counts [cells][2] += 1 at column 0 when end - start < free_ub, else at column 1 when < mono_ub. */
+int64_t mub_frag_tile_bytes(void);
+int mub_frag_newline_count(const uint8_t* text, int64_t n_bytes, int64_t* tile_counts, mub_stream_t stream);
+int mub_frag_newline_fill(const uint8_t* text, int64_t n_bytes, const int64_t* tile_offsets, int64_t* nl_pos,
+                          mub_stream_t stream);
+int mub_frag_barcode_table(const uint8_t* bc, const int64_t* bc_off, int32_t n_bc, uint64_t* keys, int32_t* slot_entry,
+                           int64_t capacity, mub_stream_t stream);
+int mub_frag_parse(const uint8_t* text, const int64_t* nl_pos, int64_t n_lines, int64_t line_base, const uint8_t* bc,
+                   const int64_t* bc_off, const int32_t* bc_val, const uint64_t* keys, const int32_t* slot_entry,
+                   int64_t capacity, int32_t* start, int32_t* end, int32_t* score, int32_t* cell, uint8_t* flags,
+                   int64_t* status, mub_stream_t stream);
+int mub_frag_overlap(const int32_t* start, const int32_t* end, const int32_t* cell, const int32_t* score,
+                     const int64_t* q_rec_lo, const int64_t* q_rec_hi, const int64_t* q_lo, const int64_t* q_hi,
+                     int32_t n_q, int64_t lmax, int32_t use_score, int32_t feat_base, int64_t* counts,
+                     const int64_t* out_off, int32_t* out_cell, int32_t* out_feat, int64_t* out_val,
+                     mub_stream_t stream);
+int mub_frag_tss_pileup(const int32_t* start, const int32_t* end, const int32_t* cell, const int32_t* score,
+                        const int64_t* q_rec_lo, const int64_t* q_rec_hi, const int64_t* q_lo, const int64_t* q_hi,
+                        int32_t n_q, int64_t lmax, int32_t width, int64_t* diff, mub_stream_t stream);
+int mub_frag_tss_rows(int64_t* diff, int64_t n_cells, int32_t width, int32_t flank, int32_t center_lo,
+                      int32_t center_hi, int64_t* sums, mub_stream_t stream);
+int mub_frag_tss_scale(const int64_t* pile, int64_t n_cells, int32_t width, const double* flank_mean, double* out,
+                       mub_stream_t stream);
+int mub_frag_nucleosome(const int32_t* start, const int32_t* end, const int32_t* cell, int64_t n, double free_ub,
+                        double mono_ub, int32_t* counts, mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -88,6 +88,15 @@ SIGNATURES = {
     "mub_rank_stats_f32": [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, i64, u32, i32, vp, i64, vp, vp],
     "mub_rank_stats_f64": [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, i64, u32, i32, vp, i64, vp, vp],
     "mub_rank_score": [vp, i32, i32, vp, i64, u32, f64, vp, vp, vp, vp, vp, vp],
+    "mub_frag_newline_count": [vp, i64, vp, vp],
+    "mub_frag_newline_fill": [vp, i64, vp, vp, vp],
+    "mub_frag_barcode_table": [vp, vp, i32, vp, vp, i64, vp],
+    "mub_frag_parse": [vp, vp, i64, i64, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp],
+    "mub_frag_overlap": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, i32, vp, vp, vp, vp, vp, vp],
+    "mub_frag_tss_pileup": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, vp, vp],
+    "mub_frag_tss_rows": [vp, i64, i32, i32, i32, i32, vp, vp],
+    "mub_frag_tss_scale": [vp, i64, i32, vp, vp, vp],
+    "mub_frag_nucleosome": [vp, vp, vp, i64, f64, f64, vp, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
@@ -98,6 +107,7 @@ SPECIAL_RESTYPE = {
     "mub_dsb_cross_workspace_bytes": ([i64, i32, i32], C.c_size_t),
     "mub_rank_shared_capacity": ([i32], i32),
     "mub_rank_workspace_slice_bytes": ([i32, i32], i64),
+    "mub_frag_tile_bytes": ([], i64),
 }
 
 TFIDF_LOG_TF, TFIDF_LOG_IDF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE, TFIDF_BINARIZE = 1, 2, 4, 8, 16

@@ -1,4 +1,5 @@
-"""``mu.atac.tl`` -- ATAC tools.  ``lsi`` and ``rank_peaks_groups`` run on the GPU; the peak annotation helpers are pandas."""
+"""``mu.atac.tl`` -- ATAC tools.  ``lsi``, ``rank_peaks_groups`` and the fragments-file tools (``count_fragments_features``,
+``tss_enrichment``, ``nucleosome_signal``) run on the GPU; the peak annotation helpers and ``locate_fragments`` are host-only."""
 from __future__ import annotations
 
 import numpy as np
@@ -252,3 +253,262 @@ def rank_peaks_groups(data, groupby, add_peak_type=False, add_distance=False, **
         raise TypeError("Expected AnnData or MuData object with 'atac' modality")
     rank_genes_groups(adata, groupby, **kwargs)
     add_genes_peaks_groups(adata, add_peak_type=add_peak_type, add_distance=add_distance)
+
+
+# ---- the fragments file (muon/_atac/tools.py:640-1201) -----------------------------------------------------------------
+def _new_anndata(X, obs, var):
+    from .._containers import SimpleAnnData, _real
+    cls = _real("AnnData", "anndata") or SimpleAnnData
+    return cls(X=X, obs=obs, var=var)
+
+
+def _gene_annotation_from_rna(data):
+    """Gene coordinates from ``mod["rna"].var["interval"]`` (``chr:start-end``), as muon/_rna/utils.py:7-37 builds
+    them: Chromosome, Start, End, gene_id, gene_name, indexed like ``var``."""
+    import pandas as pd
+    var = data.mod["rna"].var
+    parts = [str(s).replace(":", "-", 1).split("-") for s in var["interval"]]
+    table = pd.DataFrame(parts, columns=["Chromosome", "Start", "End"], index=var.index)
+    table["gene_id"] = var["gene_ids"].values
+    table["gene_name"] = var.index.values
+    table = table.loc[~table["Start"].isnull()]
+    table["Start"] = table["Start"].astype(int)
+    table["End"] = table["End"].astype(int)
+    return table
+
+
+def _features_or_rna(data, features):
+    if features is not None:
+        return features
+    if is_mudata(data) and "rna" in data.mod and "interval" in data.mod["rna"].var.columns:
+        return _gene_annotation_from_rna(data)
+    raise ValueError("Argument `features` is required. It should be a BED-like DataFrame with gene coordinates and "
+                     "names.")
+
+
+def _fragments_path(adata):
+    if "files" not in adata.uns or "fragments" not in adata.uns["files"]:
+        raise KeyError("There is no fragments file located yet. Run muon.atac.tl.locate_fragments first.")
+    return adata.uns["files"]["fragments"]
+
+
+def _integral(v, what):
+    """A fetch bound as int64: integral floats are accepted (the default extension 2e3 makes them floats)."""
+    a = np.asarray(v, dtype=np.float64) if np.asarray(v).dtype.kind == "f" else np.asarray(v)
+    if a.dtype.kind == "f":
+        if not np.all(np.isfinite(a)) or not np.all(a == np.floor(a)):
+            raise TypeError(f"{what} must be integral")
+    return a.astype(np.int64)
+
+
+def _check_fetch(contig, lo, hi):
+    """pysam's refusals of a region, before any device work: start > stop, start < 0."""
+    bad = np.flatnonzero(lo > hi)
+    if len(bad):
+        i = bad[0]
+        raise ValueError(f"invalid coordinates: start ({lo[i]}) > stop ({hi[i]})")
+    bad = np.flatnonzero(lo < 0)
+    if len(bad):
+        raise ValueError(f"start out of range ({lo[bad[0]]})")
+    if np.any(hi > (1 << 31) - 1):
+        raise NotImplementedError("fetch bounds beyond int32 are not supported")
+
+
+def _barcode_rows(adata, barcodes):
+    """Barcode -> obs row as the reference's dict builds it: the ``barcodes`` column when it exists, else obs_names;
+    a repeated barcode maps to its last row."""
+    keys = adata.obs.loc[:, barcodes] if barcodes and barcodes in adata.obs.columns else adata.obs.index
+    if len(keys) > (1 << 31) - 1:
+        raise NotImplementedError("more than 2^31 - 1 cells")
+    return {k: v for v, k in enumerate(keys)}
+
+
+def _device():
+    import torch
+    if not torch.cuda.is_available():
+        from .._lib import MuonB200Error
+        raise MuonB200Error("the fragments tools run on a CUDA device and none is available")
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def locate_fragments(data, fragments, return_fragments=False):
+    """Record the fragments file in ``uns["files"]["fragments"]`` -- drop-in for ``muon.atac.tl.locate_fragments``
+    (reference muon/_atac/tools.py:640-690).  Like the reference, any exception is printed and the call returns None.
+
+    Deliberate divergence: the path is recorded when the file opens; neither pysam nor a ``.tbi`` index is needed.
+    ``return_fragments=True`` returns ``pysam.TabixFile(fragments, parser=pysam.asBed())``, which does need pysam."""
+    try:
+        adata = _atac_of(data)
+        with open(fragments, "rb"):
+            pass
+        if "files" not in adata.uns:
+            adata.uns["files"] = dict()
+        adata.uns["files"]["fragments"] = fragments
+        if return_fragments:
+            try:
+                import pysam
+            except ImportError:
+                raise ImportError("pysam is not available. It is required to return a connection to the fragments "
+                                  "file. Install pysam from PyPI (`pip install pysam`).")
+            return pysam.TabixFile(fragments, parser=pysam.asBed())
+    except Exception as e:   # noqa: BLE001 -- the reference prints every failure
+        print(e)
+
+
+def count_fragments_features(data, features=None, stranded=False, extend_upstream=2e3, extend_downstream=0,
+                             count_reads=True, *, chunk_bytes=None):
+    """Count the fragments overlapping each feature -- drop-in for ``muon.atac.tl.count_fragments_features``
+    (reference muon/_atac/tools.py:746-891).  Returns a cells x features AnnData (``obs`` = the ATAC obs, ``var`` =
+    ``features``) whose X is a canonical int64 CSR: duplicates summed, indices sorted (the reference returns a CSC with
+    duplicate, unsorted entries; the two are equal once densified).
+
+    The whole file is parsed on the device (``muon_b200._fragments``); one warp per feature window counts the
+    overlapping fragments.  Each fragment adds ``int(score)`` (``count_reads``) or 1.  The window is ``[start -
+    extend_upstream, end + extend_downstream)`` for every feature: as in the reference, ``stranded`` is replaced by
+    whether a ``Strand`` column exists and the strand is read from the chromosome column, so no feature is ever
+    treated as on the ``-`` strand, and a ``Strand`` column with ``stranded=False`` raises KeyError.  A window starting
+    below 0 or on a contig the file lacks raises ValueError, as pysam's fetch does.  Non-unique ``obs_names`` raise
+    ValueError.  ``chunk_bytes`` (keyword-only) sets the text per device chunk."""
+    import warnings
+
+    from .. import _fragments as F
+
+    adata = _atac_of(data)
+    features = _features_or_rna(data, features)
+    path = _fragments_path(adata)
+    if count_reads:
+        warnings.warn("From v0.2, by default, unique fragments will be counted instead of reads. See muon#110 for "
+                      "details.", FutureWarning, stacklevel=2)
+    names = [str(c).lower() for c in features.columns.values]
+    for col in ("start", "end"):
+        if col not in names:
+            raise ValueError(f"No column with feature {col}s could be found")
+    chrom = next((c for c in ("chromosome", "chrom", "chr") if c in names), None)
+    if chrom is None:
+        raise ValueError("No column with chromosome for features could be found")
+    column = {key: features.columns.values[names.index(key)] for key in ("start", "end", chrom)}
+    strand_col = None
+    if stranded:
+        if "strand" not in names:
+            raise ValueError("No column with strand for features could be found")
+        strand_col = column[chrom]                       # the reference reads the strand from the chromosome column
+    stranded = "Strand" in features.columns
+    if stranded and strand_col is None and features.shape[0]:
+        raise KeyError(None)
+    contig = [str(c) for c in features[column[chrom]].values]
+    start = _integral(features[column["start"]].values, "start")
+    end = _integral(features[column["end"]].values, "end")
+    minus = np.asarray(features[strand_col].values == "-", dtype=bool) if stranded else np.zeros(len(contig), bool)
+    up, down = extend_upstream, extend_downstream
+    lo = np.where(minus, _integral(start - down, "start"), _integral(start - up, "start"))
+    hi = np.where(minus, _integral(end + up, "end"), _integral(end + down, "end"))
+    _check_fetch(contig, lo, hi)
+    if not adata.obs.index.is_unique:
+        raise ValueError("count_fragments_features needs unique obs_names")
+    index_of = _barcode_rows(adata, None)
+
+    device = _device()
+    R = F.read_records(path, index_of, device, chunk_bytes=chunk_bytes or F.CHUNK_BYTES)
+    missing = [c for c in dict.fromkeys(contig) if c not in R.contigs]
+    if missing:
+        raise ValueError(f"could not create iterator for region '{missing[0]}': contig not in the fragments file")
+    X = F.count_matrix(R, list(zip(contig, lo.tolist(), hi.tolist())), adata.n_obs, count_reads, device)
+    return _new_anndata(X, adata.obs, features)
+
+
+def tss_enrichment(data, features=None, extend_upstream=1000, extend_downstream=1000, n_tss=2000, return_tss=True,
+                   random_state=None, barcodes=None, *, use_index=True, chunk_bytes=None):
+    """TSS enrichment per cell (ENCODE) -- drop-in for ``muon.atac.tl.tss_enrichment`` (reference
+    muon/_atac/tools.py:894-1106).  Adds ``obs["tss_score"]`` and returns (``return_tss``) an AnnData whose X is the
+    cells x positions pileup divided by each cell's flank mean (float64) and whose ``var`` holds ``TSS_position``.
+
+    More than ``n_tss`` features are sampled with ``features.sample(n=n_tss, random_state=random_state)``, as in the
+    reference; features on contigs the file lacks are dropped.  Fragments with score s add s to the positions they
+    cover in ``[Start - extend_upstream, Start + extend_downstream]``.  Flanks are the first and last 100 positions,
+    the centre the middle 1001 (empty, hence NaN scores, when the region is exactly 1001 wide; ValueError when it is
+    narrower); a zero flank mean is replaced by the mean over cells.
+
+    With ``<file>.tbi`` present (``use_index``, keyword-only) only the windows are read, through the tabix linear
+    index; otherwise the whole file is parsed.  The pileup is an exact int64 difference array on the device."""
+    import warnings
+
+    import pandas as pd
+
+    from .. import _fragments as F
+
+    adata = _atac_of(data)
+    features = _features_or_rna(data, features)
+    if features.shape[0] > n_tss:
+        features = features.sample(n=n_tss, random_state=random_state)
+    path = _fragments_path(adata)
+    n = adata.n_obs
+    width = extend_downstream + extend_upstream + 1
+    index_of = _barcode_rows(adata, barcodes)
+    device = _device()
+    tbi = F.contigs_of(path) if use_index else None
+    R = None
+    if tbi is not None:
+        chromosomes = list(tbi)
+    else:
+        R = F.read_records(path, index_of, device, chunk_bytes=chunk_bytes or F.CHUNK_BYTES)
+        chromosomes = list(R.contigs)
+    features = features[features.Chromosome.isin(chromosomes)]
+    contig = [str(c) for c in features.Chromosome.values]
+    tss_start = np.asarray(features.Start.values, dtype=np.int64)
+    lo, hi = tss_start - extend_upstream, tss_start + extend_downstream
+    _check_fetch(contig, lo, hi)
+    if width < 1001:
+        raise ValueError(f"`center_size` (1001) must smaller than the piled up region ({width}).")
+    if R is None:
+        text = F.indexed_text(path, list(zip(contig, lo.tolist(), hi.tolist())), tbi)
+        chunks = F.text_chunks([text] if text else [], chunk_bytes or F.CHUNK_BYTES) if text is not None else None
+        if chunks is None:
+            R = F.read_records(path, index_of, device, chunk_bytes=chunk_bytes or F.CHUNK_BYTES)
+        else:
+            R = F.parse_chunks(chunks, F.BarcodeTable(index_of, device), device)
+    diff, sums, center_n = F.tss_pileup(R, list(zip(contig, tss_start.tolist())), n, extend_upstream,
+                                        extend_downstream, device)
+    sums = sums.cpu().numpy()
+    flank = sums[:, 0].astype(np.float64) / 200
+    flank[flank == 0] = flank.mean()
+    with np.errstate(invalid="ignore", divide="ignore"):
+        center = sums[:, 1].astype(np.float64) / center_n
+        if center_n == 0:
+            warnings.warn("Mean of empty slice.", RuntimeWarning, stacklevel=2)
+        scores = center / flank
+    X = F.tss_scale(diff, n, width, flank, device).cpu().numpy() if return_tss else None
+    adata.obs["tss_score"] = scores
+    if return_tss:
+        anno = pd.DataFrame({"TSS_position": range(-extend_upstream, extend_downstream + 1)})
+        anno.index = anno.index.astype(str)
+        return _new_anndata(X, adata.obs.copy(), anno)
+    return None
+
+
+def nucleosome_signal(data, n=None, nucleosome_free_upper_bound=147, mononuleosomal_upper_bound=294, barcodes=None,
+                      *, chunk_bytes=None):
+    """Ratio of mono-nucleosomal to nucleosome-free fragments per cell -- drop-in for ``muon.atac.tl.nucleosome_signal``
+    (reference muon/_atac/tools.py:1109-1201).  Writes ``obs["nucleosome_signal"]`` and returns None.
+
+    The first ``n`` records of the file (default ``n_obs * 1e4``) are counted, those of barcodes outside obs
+    included; a fragment shorter than ``nucleosome_free_upper_bound`` is nucleosome-free, else one shorter than
+    ``mononuleosomal_upper_bound`` is mono-nucleosomal.  Cells with no nucleosome-free fragment get one more of each.
+    A file with fewer than ``n`` records raises StopIteration, as the reference's ``next()`` does.  Reading stops as
+    soon as ``n`` records are parsed."""
+    from .. import _fragments as F
+
+    adata = _atac_of(data)
+    path = _fragments_path(adata)
+    index_of = _barcode_rows(adata, barcodes)
+    n = int(adata.n_obs * 1e4) if n is None else int(n)
+    mat = np.zeros((adata.n_obs, 2), dtype=np.int64)
+    if n > 0:
+        device = _device()
+        R = F.read_records(path, index_of, device, max_records=n, chunk_bytes=chunk_bytes or F.CHUNK_BYTES)
+        if R.n < n:
+            raise StopIteration
+        mat += F.nucleosome_counts(R, n, adata.n_obs, nucleosome_free_upper_bound, mononuleosomal_upper_bound,
+                                   device).cpu().numpy()
+    mat[mat[:, 0] == 0, :] += 1
+    adata.obs["nucleosome_signal"] = mat[:, 1] / mat[:, 0]
+    return None

@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 104; /* 0.1.4: differential accessibility (rank_peaks_groups) */ }
+int mub_version(void) { return 105; /* 0.1.5: fragments file (count_fragments_features, tss_enrichment, nucleosome_signal) */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 
