@@ -527,6 +527,51 @@ int mub_frag_tss_scale(const int64_t* pile, int64_t n_cells, int32_t width, cons
 int mub_frag_nucleosome(const int32_t* start, const int32_t* end, const int32_t* cell, int64_t n, double free_ub,
                         double mono_ub, int32_t* counts, mub_stream_t stream);
 
+/* ---- similarity network fusion (muon.tl.snf), float64 -------------------------------------------------------------
+ * Dense N x N row-major matrices on the device.  A fused state is a raw bit-symmetric X with r[i] = sum_j X[i,j] -
+ * X[i,i] (0 -> 1); its normalised matrix nv(X)[i,j] = 0.5 on the diagonal, else (X/(2 r_i) + X/(2 r_j)) / 2.  A null
+ * r anywhere below means "X is used as is".
+ *   symmetrise : D = (D + D^T) / 2 with a zero diagonal, in place.
+ *   densify    : out = the canonical CSR (indptr, indices, data) as a dense matrix, unstored entries +inf, diagonal 0.
+ *   select     : per row the k entries first in (value, column) order, ascending for SMALLEST (values X), DIST
+ *                (0.5 - nv(X), zeros skipped) and CONN (nv(X), zeros skipped), descending value for LARGEST (nv(X)).
+ *                out_idx / out_val [n x k] in that order; rows with fewer candidates are padded with -1 / 0 and
+ *                out_count[i] (may be null) says how many are real.  k <= MUB_SNF_MAX_NEIGHBORS + 1.
+ *   affinity   : means[i] = mean of the finite values of sel[i, 1..k] (sel is [n x (k+1)], the k+1 smallest of D's
+ *                row) + eps; then in place D[i,j] = exp(-(y^2)/2) / sqrt(2 pi) / s with s = sigma ((m_i + m_j)/3 +
+ *                D[i,j]/3 + eps), y = D[i,j] / s, and 0 where D[i,j] is +inf.
+ *   rowsum     : r as above, fixed-order reduction.
+ *   average    : out = (nv(xs[0]) + ... + nv(xs[count-1])) / div, summed in that order; xs / rs are host arrays of
+ *                device pointers (rs[q] may be null); out may alias xs[0] only when count == 1.
+ *   dominate   : (ptr, col, val) is the transposed top-k structure (row i lists the c with i in c's top k, ascending,
+ *                val = nv(W)[c, i]); cs[i] = the sum of row i, out[e] = val[e] / cs[col[e]].
+ *   diffuse    : C = S . B with S the CSR (s_ptr, s_col, s_val) and B read through nv(., rB).  TRANSPOSED writes
+ *                out = C^T; SYMMETRIC computes the upper triangle of C and mirrors it, so out is bit-symmetric.
+ *                B and out must not alias.  No float atomics: every call returns the same bits. */
+#define MUB_SNF_MAX_NEIGHBORS 255
+#define MUB_SNF_MAX_MODALITIES 16
+#define MUB_SNF_MAX_CELLS 1048576
+#define MUB_SNF_SELECT_SMALLEST 0
+#define MUB_SNF_SELECT_LARGEST 1
+#define MUB_SNF_SELECT_DIST 2
+#define MUB_SNF_SELECT_CONN 3
+#define MUB_SNF_DIFFUSE_TRANSPOSED 0
+#define MUB_SNF_DIFFUSE_SYMMETRIC 1
+int mub_snf_symmetrise_f64(double* D, int64_t n, mub_stream_t stream);
+int mub_snf_densify_f64(const int64_t* indptr, const int32_t* indices, const double* data, int64_t n, double* out,
+                        mub_stream_t stream);
+int mub_snf_select_f64(const double* X, const double* r, int64_t n, int32_t k, int32_t mode, int32_t* out_idx,
+                       double* out_val, int32_t* out_count, mub_stream_t stream);
+int mub_snf_affinity_f64(double* D, int64_t n, const double* sel, int32_t k, double sigma, double eps, double* means,
+                         mub_stream_t stream);
+int mub_snf_rowsum_f64(const double* X, int64_t n, double* r, mub_stream_t stream);
+int mub_snf_average_f64(const double* const* xs, const double* const* rs, int32_t count, double div, int64_t n,
+                        double* out, mub_stream_t stream);
+int mub_snf_dominate_f64(const int64_t* ptr, const int32_t* col, const double* val, int64_t n, double* cs,
+                         double* out, mub_stream_t stream);
+int mub_snf_diffuse_f64(const int64_t* s_ptr, const int32_t* s_col, const double* s_val, int64_t n, const double* B,
+                        const double* rB, double* out, int32_t mode, mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

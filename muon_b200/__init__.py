@@ -6,6 +6,7 @@
     mu.tl.mofa(mdata)            # muon/_core/tools.py:290
     mu.pp.neighbors(mdata)       # muon/_core/preproc.py:264  (WNN; first version, exact search)
     mu.prot.pp.dsb(mdata, raw)   # muon/_prot/preproc.py:17   (DSB; per-cell mixture fits on the GPU)
+    mu.tl.snf(mdata)             # muon/_core/tools.py:716   (similarity network fusion; float64 diffusion on the GPU)
     mu.tl.umap(mdata)            # muon/_core/tools.py:1209  (UMAP layout; Jacobi SGD epochs on the GPU)
     mu.atac.tl.rank_peaks_groups(atac, "leiden")   # muon/_atac/tools.py:337  (t-test / Wilcoxon per peak on the GPU)
 

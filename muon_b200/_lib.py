@@ -97,6 +97,14 @@ SIGNATURES = {
     "mub_frag_tss_rows": [vp, i64, i32, i32, i32, i32, vp, vp],
     "mub_frag_tss_scale": [vp, i64, i32, vp, vp, vp],
     "mub_frag_nucleosome": [vp, vp, vp, i64, f64, f64, vp, vp],
+    "mub_snf_symmetrise_f64": [vp, i64, vp],
+    "mub_snf_densify_f64": [vp, vp, vp, i64, vp, vp],
+    "mub_snf_select_f64": [vp, vp, i64, i32, i32, vp, vp, vp, vp],
+    "mub_snf_affinity_f64": [vp, i64, vp, i32, f64, f64, vp, vp],
+    "mub_snf_rowsum_f64": [vp, i64, vp, vp],
+    "mub_snf_average_f64": [C.POINTER(vp), C.POINTER(vp), i32, f64, i64, vp, vp],
+    "mub_snf_dominate_f64": [vp, vp, vp, i64, vp, vp, vp],
+    "mub_snf_diffuse_f64": [vp, vp, vp, i64, vp, vp, vp, i32, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
@@ -118,6 +126,9 @@ UMAP_MAX_COMPONENTS = 16
 LEIDEN_MAX_LAYERS = 4
 RANK_WILCOXON, RANK_VS_GROUP, RANK_TIE_CORRECT, RANK_OVERESTIM_VAR = 1, 2, 4, 8
 RANK_MAX_GROUPS = 1024
+SNF_MAX_NEIGHBORS, SNF_MAX_MODALITIES, SNF_MAX_CELLS = 255, 16, 1048576
+SNF_SELECT_SMALLEST, SNF_SELECT_LARGEST, SNF_SELECT_DIST, SNF_SELECT_CONN = 0, 1, 2, 3
+SNF_DIFFUSE_TRANSPOSED, SNF_DIFFUSE_SYMMETRIC = 0, 1
 
 
 class MuonB200Error(RuntimeError):
@@ -154,7 +165,8 @@ def load():
 KERNELS_PER_CALL = {"mub_csr_transpose_fill_tiled": 2, "mub_csr_transpose_fill": 2, "mub_csr_transpose_fill_f64": 2, "mub_csr_transpose_fill_pairs": 2, "mub_gram_f32": 2, "mub_version": 0, "mub_device_info": 0,
                     "mub_tfidf_tile_rows": 0, "mub_stager_create": 0, "mub_stager_destroy": 0, "mub_stager_h2d": 0, "mub_stager_d2h": 0, "mub_host_fingerprint": 0,
                     "mub_dsb_moments_f32": 4, "mub_dsb_moments_f64": 4, "mub_dsb_cross_f32": 2, "mub_dsb_cross_f64": 2,
-                    "mub_leiden_max_shared_degree": 0}
+                    "mub_leiden_max_shared_degree": 0,
+                    "mub_snf_affinity_f64": 2, "mub_snf_dominate_f64": 2}
 LAUNCHES = 0          # running count of kernels launched through this binding
 PROFILE = None        # None, or dict name -> list[(start_event, end_event)] filled by call()
 

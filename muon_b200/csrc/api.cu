@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 105; /* 0.1.5: fragments file (count_fragments_features, tss_enrichment, nucleosome_signal) */ }
+int mub_version(void) { return 106; /* 0.1.6: similarity network fusion (snf) */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 

@@ -1,4 +1,5 @@
-"""``mu.tl`` -- multimodal tools.  ``mofa`` (SURVEY section 8, rows a9-a11) and ``umap`` run on the GPU."""
+"""``mu.tl`` -- multimodal tools.  ``mofa`` (SURVEY section 8, rows a9-a11), ``snf``, ``umap``, ``leiden`` and ``louvain``
+run on the GPU."""
 from __future__ import annotations
 
 
@@ -24,3 +25,9 @@ def louvain(data, *args, **kwargs):
     """Multiplex Louvain clustering on the GPU -- drop-in for ``muon.tl.louvain`` (muon/_core/tools.py:1133)."""
     from ._leiden import louvain as _impl
     return _impl(data, *args, **kwargs)
+
+
+def snf(mdata, *args, **kwargs):
+    """Similarity network fusion on the GPU -- drop-in for ``muon.tl.snf`` (muon/_core/tools.py:716-920)."""
+    from ._snf import snf as _impl
+    return _impl(mdata, *args, **kwargs)
