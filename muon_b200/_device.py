@@ -759,9 +759,10 @@ def spmm(A, B: torch.Tensor, out: Optional[torch.Tensor] = None, accumulate=Fals
     """K2/K3: C[n x P] (+)= A @ B[d x P];  P = B.shape[1] must be 32, 64 or 128.  A is a ``DeviceCSR`` or
     ``DevicePairs``.  B is float32, or float16 holding B * ``scale`` (``to_half_scaled``): half the bytes per non-zero
     through the L2 -> L1 gather path that bounds the fp32 operand; products and sums stay fp32.  A matrix whose rows
-    are sorted (``A.sorted_indices``) is flagged so to the library, which then runs a fp32 product on CSR arrays with
-    the tiled kernel (B staged in shared memory); everything else takes the row-warp kernel (``dynamic``: rows claimed
-    from an atomic counter).  Both give the same bits."""
+    are sorted (``A.sorted_indices``) is flagged so to the library, which then runs a fp32 product of at least one
+    128-row band per SM with the tiled kernel (B staged in shared memory), on CSR arrays and on pairs alike;
+    everything else takes the row-warp kernel (``dynamic``: rows claimed from an atomic counter).  Both give the same
+    bits."""
     n, d = A.shape
     P = B.shape[1]
     assert B.shape[0] == d and B.dtype in (torch.float32, torch.float16) and B.is_contiguous(), (B.shape, d, B.dtype)

@@ -16,13 +16,15 @@
 // Traffic model (DESIGN.md): HBM streams 8 B/nnz (+ dense operands once); every non-zero
 // additionally pulls P * sizeof(T) bytes of B through L2->L1, which is the practical limiter at P>=32.
 //
-// "Tiled" kernel, for CSR arrays whose rows are known to be sorted by column and the fp32 operand: a CTA owns a band of kTiledRows consecutive rows and sweeps
-// B in column tiles (TC consecutive rows of B, one contiguous slab), each staged once into shared memory by a 1-D
-// bulk copy (TMA) and shared by every row of the band.  Each operand row then leaves L2 once per band instead of once
-// per non-zero, and the gathers are served from shared memory.  A warp keeps W rows' accumulators in registers and
-// a 32-entry window of each row's (index, value) stream; the ballot of "column < tile end" over the window gives the
-// row's segment in the tile.  Entry q of a row goes to lane group q mod G in ascending q, as in the row-warp kernel,
-// and the butterfly and store are the same: both kernels return the same bits.
+// "Tiled" kernel, for rows known to be sorted by column (CSR arrays or pairs) and the fp32 operand: a CTA owns a band
+// of kTiledRows consecutive rows and sweeps B in column tiles (TC consecutive rows of B, one contiguous slab), each
+// staged once into shared memory by a 1-D bulk copy (TMA) and shared by every row of the band.  Each operand row then
+// leaves L2 once per band instead of once per non-zero, and the gathers are served from shared memory.  A warp keeps
+// W rows' accumulators in registers and a 32-entry window of each row's (index, value) stream; the ballot of
+// "column < tile end" over the window gives the row's segment in the tile.  The band's rows go to the warps by length
+// (longest first, dealt snake-wise), so that no warp holds up the release of every tile.  Entry q of a row goes to
+// lane group q mod G in ascending q, as in the row-warp kernel, and the butterfly and store are the same: a row's
+// sum does not depend on the warp that owns it, and both kernels return the same bits.
 //
 // Half operand: every non-zero gathers half the bytes of the fp32 kernel.  Products and sums are fp32
 // (half -> float conversion is exact), only the operand is rounded (2^-11 relative).  Used by the early
@@ -202,17 +204,17 @@ static int launch_spmm(const int64_t* indptr, const int32_t* indices, const floa
 }
 
 // ---- tiled kernel ------------------------------------------------------------------------------------------------
-// CSR arrays and the fp32 operand only (see spmm_entry).  16 warps x 8 rows = a band of 128 rows per CTA, one CTA per SM (512 threads, <= 128 registers
-// each: a row's partial sums are 4 registers per lane).  Two stages of kTiledStageBytes: TC = kTiledStageBytes / (4 P)
-// rows of B per tile.  The kernel's time is a fixed part plus a cost per (row, tile) segment, so the tiles are as tall
-// as two stages allow next to the L1 that caches the entry windows.
+// Sorted rows and the fp32 operand only (see spmm_entry).  NW warps x W rows = a band of 128 rows per CTA, one CTA per
+// SM (NW * 32 threads; a row's partial sums are 4 registers per lane).  Two stages of kTiledStageBytes: TC =
+// kTiledStageBytes / (4 P) rows of B per tile.  The kernel's time is a fixed part plus a cost per (row, tile) segment,
+// so the tiles are as tall as two stages allow next to the L1 that caches the entry windows.
 constexpr int kTiledWarps = 16;
-constexpr int kTiledThreads = kTiledWarps * kWarp;
 constexpr int kTiledRowsPerWarp = 8;
-constexpr int kTiledRows = kTiledWarps * kTiledRowsPerWarp;
+constexpr int kTiledRows = 128;
 constexpr int kTiledStages = 2;
 constexpr int kTiledStageBytes = 96 << 10;  // TC = 384 rows of B at P = 64: ~12 entries per segment at 3 % density
 constexpr int kTiledSmemBytes = kTiledStages * kTiledStageBytes;
+static_assert(kTiledWarps * kTiledRowsPerWarp == kTiledRows, "a band is NW x W rows");
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count) {
@@ -237,14 +239,59 @@ __device__ __forceinline__ void tma_load_1d(void* dst, const void* src, unsigned
 
 // lane j <- entry pos + j of the row [start, start + len), column INT_MAX past the row's end.  Cached loads: the part
 // of the window a tile does not consume is read again at the next tile
+template <bool PAIRS>
 __device__ __forceinline__ void load_window(const int32_t* __restrict__ indices, const float* __restrict__ data,
                                             int64_t start, int pos, int len, int lane, int& c, float& v) {
     c = INT_MAX;
     v = 0.f;
     if (pos + lane < len) {
-        c = __ldg(indices + start + pos + lane);
-        v = __ldg(data + start + pos + lane);
+        if constexpr (PAIRS) {
+            const int2 e = __ldg(reinterpret_cast<const int2*>(indices) + start + pos + lane);
+            c = e.x;
+            v = __int_as_float(e.y);
+        } else {
+            c = __ldg(indices + start + pos + lane);
+            v = __ldg(data + start + pos + lane);
+        }
     }
+}
+
+// The band's rows dealt to warps by length: rank the R rows from the longest down (ties: lower row first; rows past
+// n_rows rank last) and deal the ranks snake-wise, rank p to warp p mod NW in even rounds and NW - 1 - p mod NW in odd
+// ones, round p / NW being the slot.  A tile is released only when every warp is done with it, so it runs at the pace
+// of the warp with the most entries in it; dealt this way each warp's rows sum to about the band's mean.  Every warp
+// ranks all R rows itself (shuffles only, no CTA barrier).  Returns, in lane w < W, the row of slot w of this warp.
+template <int NW, int W>
+__device__ __forceinline__ int64_t band_row_of_slot(const int64_t* __restrict__ indptr, int64_t n_rows, int64_t band0,
+                                                    int warp, int lane) {
+    constexpr int K = NW * W / 32;  // rows per lane: lane l holds band rows l, l + 32, ...
+    int len[K], rank[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        const int64_t r = band0 + lane + 32 * k;
+        len[k] = r < n_rows ? (int)(__ldg(indptr + r + 1) - __ldg(indptr + r)) : -1;
+        rank[k] = 0;
+    }
+#pragma unroll
+    for (int kk = 0; kk < K; ++kk) {
+        for (int src = 0; src < 32; ++src) {
+            const int lj = __shfl_sync(0xffffffffu, len[kk], src);
+            const int j = src + 32 * kk;
+#pragma unroll
+            for (int k = 0; k < K; ++k) rank[k] += (lj > len[k]) | ((lj == len[k]) & (j < lane + 32 * k));
+        }
+    }
+    int64_t row = 0;
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+        const int p = w * NW + ((w & 1) ? NW - 1 - warp : warp);
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            const unsigned m = __ballot_sync(0xffffffffu, rank[k] == p);
+            if (m != 0u && lane == w) row = band0 + 32 * k + __ffs(m) - 1;
+        }
+    }
+    return row;
 }
 
 // window lanes [0, cnt) hold row entries pos .. pos + cnt - 1, all in the staged tile (first row of B: lo):
@@ -275,17 +322,18 @@ __device__ __forceinline__ void gather_segment(float* acc, const T* __restrict__
     }
 }
 
-template <int P>
-__global__ void __launch_bounds__(kTiledThreads, 1)
+// PAIRS: interleaved (column, value) pairs, as in the row-warp kernel (the transposed panels)
+template <int P, bool PAIRS, int NW, int W>
+__global__ void __launch_bounds__(NW * kWarp, 1)
 spmm_csr_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
                       const float* __restrict__ data, int64_t n_rows, int n_cols, const float* __restrict__ B,
                       float* __restrict__ C, int accumulate) {
     using T = float;
     constexpr int VEC = 16 / sizeof(T);
     constexpr int TC = kTiledStageBytes / (P * (int)sizeof(T));
-    constexpr int W = kTiledRowsPerWarp;
-    constexpr int R = kTiledRows;
+    constexpr int R = NW * W;
     constexpr int S = kTiledStages;
+    static_assert(R % 32 == 0 && W <= 32, "band rows are ranked 32 per lane slot");
     extern __shared__ __align__(128) unsigned char stages[];
     __shared__ __align__(8) uint64_t full[S], empty[S];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -302,7 +350,7 @@ spmm_csr_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], kTiledWarps);
+            mbar_init(&empty[s], NW);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         for (int64_t i = 0; i < S && i < items; ++i) issue(i);
@@ -312,24 +360,25 @@ spmm_csr_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
     float acc[W][VEC];
     int c[W];        // window of row w: lane j holds entry rpos(w) + j
     float v[W];
-    int64_t rstart = 0;  // lane w < W: first entry, length and consumed entries of row w
+    int64_t row = 0;     // lane w < W: the row of slot w, its first entry, length and consumed entries
+    int64_t rstart = 0;
     int rlen = 0, rpos = 0;
-    int64_t row0 = 0;
     for (int64_t i = 0; i < items; ++i) {
         const int tile = (int)(i % n_tiles);
         if (tile == 0) {
-            row0 = (blockIdx.x + i / n_tiles * gridDim.x) * (int64_t)R + warp * W;
+            const int64_t band0 = (blockIdx.x + i / n_tiles * gridDim.x) * (int64_t)R;
+            row = band_row_of_slot<NW, W>(indptr, n_rows, band0, warp, lane);
             rstart = 0;
             rlen = rpos = 0;
-            if (lane < W && row0 + lane < n_rows) {
-                rstart = __ldg(indptr + row0 + lane);
-                rlen = (int)(__ldg(indptr + row0 + lane + 1) - rstart);
+            if (lane < W && row < n_rows) {
+                rstart = __ldg(indptr + row);
+                rlen = (int)(__ldg(indptr + row + 1) - rstart);
             }
 #pragma unroll
             for (int w = 0; w < W; ++w) {
 #pragma unroll
                 for (int e = 0; e < VEC; ++e) acc[w][e] = 0.f;
-                load_window(indices, data, __shfl_sync(0xffffffffu, rstart, w), 0,
+                load_window<PAIRS>(indices, data, __shfl_sync(0xffffffffu, rstart, w), 0,
                                    __shfl_sync(0xffffffffu, rlen, w), lane, c[w], v[w]);
             }
         }
@@ -348,7 +397,7 @@ spmm_csr_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
             for (;;) {
                 gather_segment<P, T>(acc[w], tl, lo, c[w], v[w], pos, cnt, lane);
                 pos += cnt;
-                load_window(indices, data, st, pos, len, lane, c[w], v[w]);
+                load_window<PAIRS>(indices, data, st, pos, len, lane, c[w], v[w]);
                 if (cnt < 32) break;  // the reload is only needed at the next tile
                 cnt = __popc(__ballot_sync(0xffffffffu, c[w] < hi));
                 if (cnt == 0) break;
@@ -365,24 +414,27 @@ spmm_csr_tiled_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
         __syncwarp();
         if (tile == n_tiles - 1) {
 #pragma unroll
-            for (int w = 0; w < W; ++w)
-                if (row0 + w < n_rows) store_row<P, T>(acc[w], C + (size_t)(row0 + w) * P, accumulate, 1.f, lane);
+            for (int w = 0; w < W; ++w) {
+                const int64_t r = __shfl_sync(0xffffffffu, row, w);
+                if (r < n_rows) store_row<P, T>(acc[w], C + (size_t)r * P, accumulate, 1.f, lane);
+            }
         }
     }
 }
 
-template <int P>
+template <int P, bool PAIRS>
 static int launch_spmm_tiled(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_rows,
                              int n_cols, const float* B, float* C, int accumulate, cudaStream_t stream,
                              const char* name) {
-    auto kernel = spmm_csr_tiled_kernel<P>;
+    auto kernel = spmm_csr_tiled_kernel<P, PAIRS, kTiledWarps, kTiledRowsPerWarp>;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTiledSmemBytes);
     MUB_REQUIRE(e == cudaSuccess, "%s: %s", name, cudaGetErrorString(e));
     const int64_t bands = (n_rows + kTiledRows - 1) / kTiledRows;
     // one CTA per SM, every CTA sweeping B at about the same pace: the tiles a CTA stages were just staged by the
     // others and are still in L2
     const int grid = (int)(bands < sm_count() ? bands : sm_count());
-    kernel<<<grid, kTiledThreads, kTiledSmemBytes, stream>>>(indptr, indices, data, n_rows, n_cols, B, C, accumulate);
+    kernel<<<grid, kTiledWarps * kWarp, kTiledSmemBytes, stream>>>(indptr, indices, data, n_rows, n_cols, B, C,
+                                                                   accumulate);
     return check_launch(name);
 }
 
@@ -400,18 +452,18 @@ static int spmm_entry(const char* name, const int64_t* indptr, const int32_t* in
     MUB_REQUIRE(!PAIRS || ((uintptr_t)indices & 7) == 0, "%s: pairs must be 8-byte aligned", name);
     const T* Bt = (const T*)B;
     cudaStream_t s = (cudaStream_t)stream;
-    // measured on the LSI products (profiles/README.md): the tiled kernel wins on A*V with the fp32 operand.  With the
-    // half operand the row-warp kernel gathers half the bytes while the tiled kernel's cost per (row, tile) segment
-    // stays; on the pairs-layout A^T panels the operand slice already sits in L2 and the rows' skewed lengths want
-    // the row-warp kernel's dynamic scheduling
-    if constexpr (std::is_same_v<T, float> && !PAIRS) {
-        if ((flags & MUB_SPMM_ROWS_SORTED) && n_cols > 0) {
+    // measured on the LSI products (profiles/README.md): with the fp32 operand the tiled kernel wins on A*V and on the
+    // pairs-layout A^T panels.  With the half operand the row-warp kernel gathers half the bytes while the tiled
+    // kernel's cost per (row, tile) segment stays.  A launch of fewer bands than SMs (the sampled row blocks of the
+    // residual check) would leave most SMs idle in the tiled kernel; the row-warp kernel spreads it over all of them
+    if constexpr (std::is_same_v<T, float>) {
+        if ((flags & MUB_SPMM_ROWS_SORTED) && n_cols > 0 && (n_rows + kTiledRows - 1) / kTiledRows >= sm_count()) {
             MUB_REQUIRE(n_cols < INT_MAX, "%s: n_cols must be below 2^31", name);
             const int d = (int)n_cols;
             switch (ld) {
-                case 32: return launch_spmm_tiled<32>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
-                case 64: return launch_spmm_tiled<64>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
-                default: return launch_spmm_tiled<128>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
+                case 32: return launch_spmm_tiled<32, PAIRS>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
+                case 64: return launch_spmm_tiled<64, PAIRS>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
+                default: return launch_spmm_tiled<128, PAIRS>(indptr, indices, data, n_rows, d, Bt, C, accumulate, s, name);
             }
         }
     }

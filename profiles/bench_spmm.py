@@ -1,7 +1,9 @@
 """Micro-benchmark of the four SpMM entry points on a slice of the bench matrix: A·B on the CSR arrays
 (mub_spmm_csr_*) and Aᵀ·B on the transposed pairs panels (mub_spmm_csrp_*), fp32 and half operand, P = 32, 64, 128.
-Every product runs twice on the same arrays: flagged sorted (mub_spmm_csr_f32 then runs the tiled kernel, the other
-entry points the row-warp kernel either way) and flagged unsorted (the row-warp kernel).  CUDA events around `reps` passes after `warmup` passes; the digest of each output lets two library builds
+Every product runs twice on the same arrays: flagged sorted (the fp32 entry points mub_spmm_csr_f32 and
+mub_spmm_csrp_f32 then run the tiled kernel, the half-operand ones the row-warp kernel either way) and flagged
+unsorted (the row-warp kernel).  CUDA events around `reps` passes after `warmup` passes; the digest of each output
+lets two library builds
 (MUON_B200_LIB) be compared bit for bit, and the largest relative difference between the two runs is printed.
     python profiles/bench_spmm.py [cells] [peaks] [reps] [P ...]"""
 import hashlib
