@@ -572,6 +572,32 @@ int mub_snf_dominate_f64(const int64_t* ptr, const int32_t* col, const double* v
 int mub_snf_diffuse_f64(const int64_t* s_ptr, const int32_t* s_col, const double* s_val, int64_t n, const double* B,
                         const double* rB, double* out, int32_t mode, mub_stream_t stream);
 
+/* ---- motif scanning (muon.atac.tl.scan_sequences), float64 -------------------------------------------------------
+ *   encode : in place, A/a C/c G/g T/t -> 0..3, every other byte -> 4.
+ *   count  : sequences are codes[seq_off[s] .. seq_off[s+1]), cut into tiles of MUB_MOTIF_TILE window starts
+ *            (tile_seq[g] = its sequence, seq_tile0[s] = the sequence's first tile).  Motif m has the columns
+ *            col_off[m] .. col_off[m+1] (length <= MUB_MOTIF_MAX_LEN) of tab, MUB_MOTIF_CODES scores per column, the
+ *            fifth -inf; motifs are scanned in groups group_m0[q] .. group_m0[q+1] of at most MUB_MOTIF_GROUP_COLS
+ *            columns.  A window's score is the float64 sum over its columns in order from 0.0; it is a hit when
+ *            score >= thr[m].  counts[seq_tile0[s] * n_motifs + m * n_tiles(s) + (g - seq_tile0[s])] = hits of motif
+ *            m in tile g, i.e. laid out in (sequence, motif, tile) order.
+ *   fill   : with offsets = the exclusive scan of counts, writes every hit (sequence, motif, window start, score) at
+ *            its offset, in (sequence, motif, position) order.  No float atomics: every call returns the same bits. */
+#define MUB_MOTIF_MAX_LEN 64
+#define MUB_MOTIF_TILE 512
+#define MUB_MOTIF_CODES 5
+#define MUB_MOTIF_GROUP_COLS 512
+int mub_motif_encode(uint8_t* bytes, int64_t n, mub_stream_t stream);
+int mub_motif_count(const uint8_t* codes, const int64_t* seq_off, const int32_t* tile_seq, const int64_t* seq_tile0,
+                    int64_t n_tiles, const double* tab, const int32_t* col_off, const double* thr,
+                    const int32_t* group_m0, int32_t n_groups, int32_t n_motifs, int32_t* counts,
+                    mub_stream_t stream);
+int mub_motif_fill(const uint8_t* codes, const int64_t* seq_off, const int32_t* tile_seq, const int64_t* seq_tile0,
+                   int64_t n_tiles, const double* tab, const int32_t* col_off, const double* thr,
+                   const int32_t* group_m0, int32_t n_groups, int32_t n_motifs, const int32_t* counts,
+                   const int64_t* offsets, int32_t* out_seq, int32_t* out_motif, int32_t* out_pos, double* out_score,
+                   mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

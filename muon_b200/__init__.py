@@ -9,6 +9,7 @@
     mu.tl.snf(mdata)             # muon/_core/tools.py:716   (similarity network fusion; float64 diffusion on the GPU)
     mu.tl.umap(mdata)            # muon/_core/tools.py:1209  (UMAP layout; Jacobi SGD epochs on the GPU)
     mu.atac.tl.rank_peaks_groups(atac, "leiden")   # muon/_atac/tools.py:337  (t-test / Wilcoxon per peak on the GPU)
+    mu.atac.tl.scan_sequences(seqs)                # muon/_atac/tools.py:446  (motif hits; every window scored on the GPU)
 
 Same signatures and AnnData/MuData slot semantics as the reference; the arithmetic runs in
 hand-written CUDA kernels behind the C ABI in include/muon_b200.h.  There is no CPU fallback.

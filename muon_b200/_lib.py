@@ -105,6 +105,9 @@ SIGNATURES = {
     "mub_snf_average_f64": [C.POINTER(vp), C.POINTER(vp), i32, f64, i64, vp, vp],
     "mub_snf_dominate_f64": [vp, vp, vp, i64, vp, vp, vp],
     "mub_snf_diffuse_f64": [vp, vp, vp, i64, vp, vp, vp, i32, vp],
+    "mub_motif_encode": [vp, i64, vp],
+    "mub_motif_count": [vp, vp, vp, vp, i64, vp, vp, vp, vp, i32, i32, vp, vp],
+    "mub_motif_fill": [vp, vp, vp, vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
@@ -129,6 +132,7 @@ RANK_MAX_GROUPS = 1024
 SNF_MAX_NEIGHBORS, SNF_MAX_MODALITIES, SNF_MAX_CELLS = 255, 16, 1048576
 SNF_SELECT_SMALLEST, SNF_SELECT_LARGEST, SNF_SELECT_DIST, SNF_SELECT_CONN = 0, 1, 2, 3
 SNF_DIFFUSE_TRANSPOSED, SNF_DIFFUSE_SYMMETRIC = 0, 1
+MOTIF_MAX_LEN, MOTIF_TILE, MOTIF_CODES, MOTIF_GROUP_COLS = 64, 512, 5, 512
 
 
 class MuonB200Error(RuntimeError):

@@ -1,5 +1,6 @@
-"""``mu.atac.tl`` -- ATAC tools.  ``lsi``, ``rank_peaks_groups`` and the fragments-file tools (``count_fragments_features``,
-``tss_enrichment``, ``nucleosome_signal``) run on the GPU; the peak annotation helpers and ``locate_fragments`` are host-only."""
+"""``mu.atac.tl`` -- ATAC tools.  ``lsi``, ``rank_peaks_groups``, the fragments-file tools (``count_fragments_features``,
+``tss_enrichment``, ``nucleosome_signal``) and ``scan_sequences`` run on the GPU; the peak annotation helpers,
+``locate_fragments``, ``locate_file``, ``locate_genome`` and ``get_sequences`` are host-only."""
 from __future__ import annotations
 
 import numpy as np
@@ -512,3 +513,104 @@ def nucleosome_signal(data, n=None, nucleosome_free_upper_bound=147, mononuleoso
     mat[mat[:, 0] == 0, :] += 1
     adata.obs["nucleosome_signal"] = mat[:, 1] / mat[:, 0]
     return None
+
+
+# ---- sequences and motifs (muon/_atac/tools.py:381-618) ------------------------------------------------------------------
+def _parse_motif_ids(filename=None):
+    """The motif_id -> tf_gene_name table (reference muon/_atac/tools.py:381-389), indexed by ``motif_id``.
+    ``filename=None`` reads ``motif_to_gene.txt`` of the JASPAR database bundled with an importable ``muon`` package;
+    without one it raises FileNotFoundError."""
+    from .._motifs import parse_motif_ids
+    return parse_motif_ids(filename)
+
+
+def _parse_motif_matrices(files=None, background=4, pseudocount=0.0001):
+    """Log-odds matrices of ``.pfm`` count files (reference muon/_atac/tools.py:392-416): ``{"motifs": ids,
+    "matrices": [float64 (4, L) arrays]}``, with ids ``os.path.basename(f).rstrip(".pfm")`` (a character-set strip, as
+    in the reference).  ``files=None`` globs the JASPAR database bundled with an importable ``muon`` package; without
+    one it raises FileNotFoundError: pass ``files=``.  A file that is not 4 rows (A, C, G, T) of counts raises
+    ValueError; so does a background that is not 4 frequencies summing to 1."""
+    from .._motifs import parse_motif_matrices
+    return parse_motif_matrices(files, background, pseudocount)
+
+
+def _prepare_motif_scanner(matrices=None, background=4, pvalue=0.0001, max_hits=10):
+    """A ``MotifScanner`` (reference muon/_atac/tools.py:419-443): the log-odds tables, per-motif lengths and
+    p-value thresholds, uploaded once to the current CUDA device.  ``max_hits`` is MOODS' lookahead window size; it
+    does not change results and is ignored.  ``pvalue`` outside (0, 1] raises ValueError; motifs longer than 64
+    columns raise NotImplementedError."""
+    from .._motifs import prepare_motif_scanner
+    return prepare_motif_scanner(matrices, background, pvalue, max_hits)
+
+
+def scan_sequences(sequences, motif_scanner=None, matrices=None, motifs=None, motif_meta=None, background=4,
+                   pvalue=0.0001, max_hits=10):
+    """Scan sequences for motif hits on the GPU -- drop-in for ``muon.atac.tl.scan_sequences`` (reference
+    muon/_atac/tools.py:446-517).
+
+    Returns a DataFrame with one row per hit, ordered by sequence, then motif (list order), then position:
+    ``sequence`` (the caller's own ``str`` objects, not copies), ``motif_id``, ``position`` (0-based window start,
+    int64) and ``score`` (float64); with ``motif_meta`` it is left-joined on ``motif_id`` (``motif_id, sequence,
+    position, score, tf_gene_name``).  Without a scanner or matrices the JASPAR database bundled with an importable
+    ``muon`` package is used, with its motif_to_gene table as ``motif_meta``.  Custom matrices with ``motif_meta=None``
+    get that table too when ``muon`` is importable; otherwise the join is skipped with a UserWarning.
+
+    Only the forward strand is scanned, as in the reference.  A window is scored as the float64 sum of its columns in
+    order; ``a/c/g/t`` score like ``A/C/G/T`` and a window holding any other character (N, IUPAC codes) is not scored.
+    A hit is ``score >= threshold``.  ``motif_scanner`` must be a ``MotifScanner`` from ``_prepare_motif_scanner``
+    (anything else, such as a MOODS scanner, raises TypeError: there is no CPU scanner); ``max_hits`` is ignored.
+    Zero hits raise ValueError, as the reference does when it names the columns of an empty frame.  Under pandas >= 3
+    the reference's frame converts ``sequence`` to the ``str`` dtype, copying every sequence; here it stays an object
+    column of the caller's strings."""
+    from .._motifs import scan_sequences as scan
+    return scan(sequences, motif_scanner, matrices, motifs, motif_meta, background, pvalue, max_hits)
+
+
+def get_sequences(data, bed, fasta_file, bed_file=None):
+    """Sequences of BED intervals from a FASTA file -- drop-in for ``muon.atac.tl.get_sequences`` (reference
+    muon/_atac/tools.py:520-566), without pybedtools.
+
+    The genome is ``uns["files"]["genome"]`` when set (``fasta_file`` is then ignored), else ``fasta_file`` is
+    recorded there first.  ``bed_file`` is read when given (``bed`` must then be None); ``bed=None`` uses the
+    features, named ``chrX:NNN-NNN``.  One sequence per interval (0-based, half-open), case preserved; an interval
+    past the end of its contig, or on a contig missing from the FASTA, is skipped with a warning, so the list can be
+    shorter than the intervals (as with bedtools).  Start > end raises ValueError.  The FASTA is read through
+    ``<fasta>.fai`` when present, else indexed in memory (no ``.fai`` is written); compressed FASTA raises
+    NotImplementedError and lines of uneven width inside a record raise ValueError."""
+    from .._motifs import get_fasta
+
+    adata = _atac_of(data)
+    if "files" not in adata.uns or "genome" not in adata.uns["files"]:
+        if fasta_file is not None:
+            locate_genome(adata, fasta_file)
+        else:
+            raise FileNotFoundError("Genome file has to be provided with `fasta_file` or located using "
+                                    "`muon.atac.tl.locate_genome`.")
+    else:
+        fasta_file = adata.uns["files"]["genome"]
+    if bed_file is not None:
+        assert bed is None
+        with open(bed_file) as fh:
+            bed = fh.read()
+    elif bed is None:
+        bed = "\n".join([i.replace(":", "-", 1).replace("-", "\t", 2) for i in adata.var.index.values])
+    return get_fasta(bed, fasta_file)
+
+
+def locate_file(data, key, file):
+    """Record ``file`` in ``uns["files"][key]`` -- drop-in for ``muon.atac.tl.locate_file`` (reference
+    muon/_atac/tools.py:569-596).  A missing file raises FileNotFoundError."""
+    import os
+    adata = _atac_of(data)
+    if not os.path.exists(file):
+        raise FileNotFoundError(f"File {file} does not exist")
+    if "files" not in adata.uns:
+        adata.uns["files"] = dict()
+    adata.uns["files"][key] = file
+
+
+def locate_genome(data, fasta_file):
+    """Record the genome FASTA in ``uns["files"]["genome"]`` -- drop-in for ``muon.atac.tl.locate_genome``
+    (reference muon/_atac/tools.py:599-618)."""
+    _atac_of(data)
+    locate_file(data, "genome", fasta_file)

@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 106; /* 0.1.6: similarity network fusion (snf) */ }
+int mub_version(void) { return 107; /* 0.1.7: motif scanning (scan_sequences) */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 
