@@ -428,6 +428,9 @@ int mub_knn_l2_tc_f32(const float* X, int64_t nq, const float* Y, int64_t nc, in
     float* kbuf = (float*)(ws + L.kbuf);
     int32_t* ibuf = (int32_t*)(ws + L.ibuf);
     cudaError_t e = cudaMemsetAsync(ymax, 0, 4, s);
+    // a CTA that sees status bit 2 skips its remaining query tiles without writing their candidate lists: the re-rank
+    // still runs on every row, so those rows must read as empty rather than as whatever the workspace held
+    if (e == cudaSuccess) e = cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)nq, s);
     if (e != cudaSuccess) {
         mub::set_error("knn_l2_tc: memset: %s", cudaGetErrorString(e));
         return -2;

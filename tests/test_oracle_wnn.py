@@ -80,3 +80,49 @@ def test_product_umap_connectivities_match_the_standin_on_cpu_tensors():
     assert (got != got.T).nnz == 0
     assert abs(got - ref).max() < 2e-5
     assert got.nnz == ref.nnz
+
+
+def _planted_isolated_clusters(seed=4, n_main=150, sizes=(5, 8, 12, 15), k=8):
+    """Two modalities; small clusters far from everything else, so that their cells share kNN neighbours with fewer
+    than n_bandwidth_neighbors = 20 cells (the bandwidth search then fills up with ties at N + 1)."""
+    rng = np.random.default_rng(seed)
+    reps, graphs = [], []
+    for d in (6, 4):
+        parts = [rng.normal(size=(n_main, d))]
+        for s in sizes:
+            u = rng.normal(size=d)
+            parts.append(40.0 * u / np.linalg.norm(u) + 0.3 * rng.normal(size=(s, d)))
+        R = np.concatenate(parts).astype(np.float32).astype(np.float64)
+        idx, dist, _ = tp.nearest_neighbors(R, k, "euclidean")
+        n = R.shape[0]
+        graphs.append(sp.csr_matrix((dist[:, 1:].ravel(), idx[:, 1:].ravel(), np.arange(0, n * (k - 1) + 1, k - 1)),
+                                    shape=(n, n)))
+        reps.append(R)
+    return reps, graphs, k
+
+
+@pytest.mark.parametrize("case", ["golden", "isolated"])
+def test_per_cell_restatement_equals_the_whole_graph_one(case):
+    """oracle/wnn_ref.py::wnn_cells_ref (everything from the cell's own row, for large N) against wnn_ref on every
+    cell: the golden, and a case whose isolated cells take the bandwidth search's fill-up path."""
+    from oracle.wnn_ref import wnn_cells_ref, wnn_ref
+    if case == "golden":
+        z = load_golden("wnn_small.npz")
+        reps, graphs, k = [z["rep_rna"], z["rep_atac"]], [golden_csr(z, "knn_rna"), golden_csr(z, "knn_atac")], \
+            int(z["n_neighbors"])
+        kw = dict(n_multineighbors=40)
+    else:
+        reps, graphs, k = _planted_isolated_clusters()
+        kw = dict(n_multineighbors=30)
+        B = sp.csr_matrix((np.ones_like(graphs[0].data), graphs[0].indices, graphs[0].indptr), shape=graphs[0].shape)
+        overlap = np.diff((B @ B.T).tocsr().indptr) - 1
+        assert (overlap < 20).sum() >= 20                       # the planted clusters reach the fill-up path
+    ref = wnn_ref(reps, graphs, k, **kw)
+    cells = np.arange(reps[0].shape[0])
+    got = wnn_cells_ref(cells, reps, graphs, k, **kw)
+    np.testing.assert_allclose(got["weights"], ref["weights"], rtol=1e-12, atol=1e-15)
+    for a, b in zip(got["sigma"], ref["sigma"]):
+        np.testing.assert_allclose(a, b, rtol=1e-12)
+    np.testing.assert_array_equal(got["knn_indices"], ref["knn_indices"])
+    np.testing.assert_allclose(got["knn_dists"], ref["knn_dists"], rtol=1e-12, atol=1e-15)
+
