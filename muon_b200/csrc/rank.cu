@@ -382,13 +382,56 @@ __device__ double beta_cf(double a, double b, double x) {
     }
     return h;
 }
+// I_x(a, 1/2) for large a, given ln x: DiDonato & Morris's BGRAT (ACM TOMS 18 (1992) 360, eq. 9), Temme's expansion
+// in powers of 1/T with T = a - 1/4 and u = -T ln x:
+//   I_x(a, b) = Gamma(a + b) / (Gamma(a) T^b) * sum_n p_n J_n(b, u),   J_0 = Gamma(b, u) / Gamma(b) = erfc(sqrt u),
+// J_n by the recursion 9.6 (held here multiplied by u^b e^-u / Gamma(b)), p_n by 9.4.  The continued fraction loses
+// about a * eps at large a; this series does not, and needs fewer terms the larger a is.
+constexpr double kBgratMinA = 300.0;             // df >= 600: the series takes <= ~20 terms up to p ~ 1e-300
+constexpr int kBgratTerms = 30;
+__device__ double beta_large_a_half(double a, double lx) {
+    const double b = 0.5, T = a - 0.25, u = -T * lx;
+    if (!(u < 745.0)) return 0.0;                  // below the smallest subnormal (and ln x = -inf)
+    const double su = sqrt(u);
+    const double h = exp(-u) * su * 0.56418958354775628695;                      // u^b e^-u / Gamma(b)
+    const double pre = exp(0.57236494292470008707 - lbeta_half(a) - 0.5 * log(T));   // Gamma(a+1/2) / (Gamma(a) sqrt T)
+    double j = erfc(su), s = j;
+    double p[kBgratTerms];
+    p[0] = 1.0;
+    const double lx2 = 0.25 * lx * lx, t4 = 4.0 * T * T;
+    double lxp = 1.0, b2n = b, fact = 1.0;        // (ln x / 2)^(2n - 2), b + 2n - 2, (2n + 1)!
+    for (int n = 1; n < kBgratTerms; ++n) {
+        fact *= (double)(2 * n) * (double)(2 * n + 1);
+        double acc = 0.0, fm = 1.0;                 // fm = (2m + 1)!
+        for (int m = 1; m < n; ++m) {
+            fm *= (double)(2 * m) * (double)(2 * m + 1);
+            acc += ((double)m * b - (double)n) * p[n - m] / fm;
+        }
+        p[n] = acc / (double)n + (b - 1.0) / fact;
+        j = (b2n * (b2n + 1.0) * j + (u + b2n + 1.0) * lxp * h) / t4;
+        lxp *= lx2;
+        b2n += 2.0;
+        const double r = p[n] * j;
+        s += r;
+        if (fabs(r) <= 1e-17 * fabs(s)) break;
+    }
+    return fmin(1.0, pre * s);
+}
 // two-sided p of Student's t with df degrees of freedom: I_{df/(df+t^2)}(df/2, 1/2)
 __device__ double student_p(double t, double df) {
     if (isnan(t) || isnan(df)) return nan("");
+    const double at = fabs(t);
+    if (isinf(at)) return 0.0;
+    if (at == 0.0) return 1.0;
     const double t2 = t * t;
-    if (isinf(t2)) return 0.0;
-    if (t2 == 0.0) return 1.0;
     const double a = 0.5 * df, b = 0.5;
+    if (a >= kBgratMinA) return beta_large_a_half(a, -log1p(t2 / df));
+    if (isinf(t2)) {
+        // |t| > 1.3e154: p ~ |t|^-df is still far above the smallest double at small df.  ln x from r = sqrt(df) / |t|.
+        const double r = sqrt(df) / at, r2 = r * r;
+        const double lx = 2.0 * log(r) - log1p(r2);
+        return exp(a * lx - b * log1p(r2) - lbeta_half(a)) * beta_cf(a, b, r2 / (1.0 + r2)) / a;
+    }
     const double x = df / (df + t2), y = t2 / (df + t2);
     const double lpre = -a * log1p(t2 / df) + b * log(y) - lbeta_half(a);
     if (x < (a + 1.0) / (a + b + 2.0)) return exp(lpre) * beta_cf(a, b, x) / a;

@@ -45,12 +45,12 @@ def _dense(X, cols):
 
 
 def tie_term(ranks):
-    """sum over tie blocks of t^3 - t, per column of a rank matrix (int64, exact)."""
-    out = np.zeros(ranks.shape[1], dtype=np.int64)
+    """sum over tie blocks of t^3 - t, per column of a rank matrix, as exact Python ints (an object array): t^3 wraps
+    int64 from t = 2 097 153 on, and the sum of a column exceeds it even earlier."""
+    out = np.zeros(ranks.shape[1], dtype=object)
     for j in range(ranks.shape[1]):
         _, t = np.unique(ranks[:, j], return_counts=True)
-        t = t.astype(np.int64)
-        out[j] = int((t**3 - t).sum())
+        out[j] = sum(int(c) ** 3 - int(c) for c in t)
     return out
 
 

@@ -68,6 +68,23 @@ def test_oracle_tie_corrected_z_equals_mannwhitneyu():
         np.testing.assert_allclose(res["pvals"][str(g)], want.pvalue[order], rtol=1e-12, atol=0)
 
 
+def test_tie_term_exact_beyond_int64():
+    """A tie block of 2 097 153 = 2^21 + 1 cells: t^3 - t is above 2^63, where int64 arithmetic wraps negative.  The
+    ranked-cell limit admits blocks up to 2 642 244 cells, so the oracle must stay exact there."""
+    t = 2_097_153
+    ranks = np.zeros((t + 3, 2))
+    ranks[t:, 0] = [1.0, 2.0, 2.0]                      # column 0: blocks of t, 1 and 2
+    ranks[:, 1] = np.arange(t + 3)                      # column 1: no ties
+    got = R.tie_term(ranks)
+    assert got[0] == t**3 - t + 2**3 - 2 and got[0] > 2**63
+    assert got[1] == 0
+    X = np.zeros((t + 3, 1))
+    X[: t + 1, 0] = 5.0                                 # a stored block of t + 1, next to a zero block of 2
+    st = R.group_stats(X, np.stack([np.arange(t + 3) < 4, np.arange(t + 3) >= 4]), None, tie_correct=True)
+    want = float((t + 1) ** 3 - (t + 1) + 2**3 - 2)
+    assert st["tie"][0, 0] == want and st["tie"][1, 0] == want
+
+
 def test_bh_and_top_selection():
     import torch
     rng = np.random.default_rng(3)
