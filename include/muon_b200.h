@@ -598,6 +598,39 @@ int mub_motif_fill(const uint8_t* codes, const int64_t* seq_off, const int32_t* 
                    const int64_t* offsets, int32_t* out_seq, int32_t* out_motif, int32_t* out_pos, double* out_score,
                    mub_stream_t stream);
 
+/* ---- independent component analysis (muon.tl.ica, muon/_core/tools.py:1365-1386: sklearn FastICA) -----------------
+ * X [n x p] row-major in the input dtype (_f32 / _f64), p <= MUB_ICA_MAX_DIM; X1 [n x k] float64 row-major.  Every
+ * sum is float64 in a fixed order (per-CTA partials in `workspace`, of mub_ica_workspace_bytes(n, p, k) bytes, summed
+ * in CTA order): every call returns the same bits.
+ *   moments : mean[p] = column means, gram[p x p] = (X - mean)^T (X - mean); *status (int32, zeroed by the caller)
+ *             gets bit0 if a value is not finite.
+ *   project : X1[i, :] = Kt^T (x_i - mean) (Kt [p x k], the whitening matrix transposed with sqrt(n) folded in); Kt ==
+ *             NULL: X1 = x widened (k == p, mean unused).  Sets bit0 of *status as moments does.
+ *   step    : one fixed-point pass for the r rows of W [r x k]: with y = W x1_i, out[r k + r] = [sum_i g(y) x1_i^T |
+ *             sum_i g'(y)] for fun LOGCOSH (g = tanh(alpha y)), EXP (y e^(-y^2/2)) or CUBE (y^3).
+ *   sources : v = T(Mt^T x1_i) (Mt [k x k], T the output type), then v = T(v / d1) and v = T(v / d2) for the non-null
+ *             divisors [k].  Exactly one of out and stats: out [n x k] = v, or stats[2k] = the column means and ddof-0
+ *             standard deviations of v (nothing written to out). */
+#define MUB_ICA_MAX_DIM 128
+#define MUB_ICA_LOGCOSH 0
+#define MUB_ICA_EXP 1
+#define MUB_ICA_CUBE 2
+size_t mub_ica_workspace_bytes(int64_t n, int32_t p, int32_t k);
+int mub_ica_moments_f32(const float* X, int64_t n, int32_t p, void* workspace, double* mean, double* gram,
+                        int32_t* status, mub_stream_t stream);
+int mub_ica_moments_f64(const double* X, int64_t n, int32_t p, void* workspace, double* mean, double* gram,
+                        int32_t* status, mub_stream_t stream);
+int mub_ica_project_f32(const float* X, int64_t n, int32_t p, const double* mean, const double* Kt, int32_t k,
+                        double* X1, int32_t* status, mub_stream_t stream);
+int mub_ica_project_f64(const double* X, int64_t n, int32_t p, const double* mean, const double* Kt, int32_t k,
+                        double* X1, int32_t* status, mub_stream_t stream);
+int mub_ica_step_f64(const double* X1, int64_t n, int32_t k, const double* W, int32_t r, int32_t fun, double alpha,
+                     void* workspace, double* out, mub_stream_t stream);
+int mub_ica_sources_f32(const double* X1, int64_t n, int32_t k, const double* Mt, const double* d1, const double* d2,
+                        float* out, void* workspace, double* stats, mub_stream_t stream);
+int mub_ica_sources_f64(const double* X1, int64_t n, int32_t k, const double* Mt, const double* d1, const double* d2,
+                        double* out, void* workspace, double* stats, mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

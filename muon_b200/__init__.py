@@ -8,6 +8,7 @@
     mu.prot.pp.dsb(mdata, raw)   # muon/_prot/preproc.py:17   (DSB; per-cell mixture fits on the GPU)
     mu.tl.snf(mdata)             # muon/_core/tools.py:716   (similarity network fusion; float64 diffusion on the GPU)
     mu.tl.umap(mdata)            # muon/_core/tools.py:1209  (UMAP layout; Jacobi SGD epochs on the GPU)
+    mu.tl.ica(mdata, basis="X_mofa")   # muon/_core/tools.py:1365  (FastICA; the passes over the cells on the GPU)
     mu.atac.tl.rank_peaks_groups(atac, "leiden")   # muon/_atac/tools.py:337  (t-test / Wilcoxon per peak on the GPU)
     mu.atac.tl.scan_sequences(seqs)                # muon/_atac/tools.py:446  (motif hits; every window scored on the GPU)
 

@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 107; /* 0.1.7: motif scanning (scan_sequences) */ }
+int mub_version(void) { return 108; /* 0.1.8: independent component analysis (ica) */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 

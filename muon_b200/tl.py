@@ -1,5 +1,5 @@
-"""``mu.tl`` -- multimodal tools.  ``mofa`` (SURVEY section 8, rows a9-a11), ``snf``, ``umap``, ``leiden`` and ``louvain``
-run on the GPU."""
+"""``mu.tl`` -- multimodal tools.  ``mofa`` (SURVEY section 8, rows a9-a11), ``snf``, ``umap``, ``leiden``, ``louvain``
+and ``ica`` run on the GPU."""
 from __future__ import annotations
 
 
@@ -31,3 +31,10 @@ def snf(mdata, *args, **kwargs):
     """Similarity network fusion on the GPU -- drop-in for ``muon.tl.snf`` (muon/_core/tools.py:716-920)."""
     from ._snf import snf as _impl
     return _impl(mdata, *args, **kwargs)
+
+
+def ica(data, *args, **kwargs):
+    """Independent component analysis (FastICA) of an ``obsm`` basis on the GPU -- drop-in for ``muon.tl.ica``
+    (muon/_core/tools.py:1365-1386)."""
+    from ._ica import ica as _impl
+    return _impl(data, *args, **kwargs)
