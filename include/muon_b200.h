@@ -631,6 +631,41 @@ int mub_ica_sources_f32(const double* X1, int64_t n, int32_t k, const double* Mt
 int mub_ica_sources_f64(const double* X1, int64_t n, int32_t k, const double* Mt, const double* d1, const double* d2,
                         double* out, void* workspace, double* stats, mub_stream_t stream);
 
+/* ---- scOpen imputation (muon.atac.pp.scopen, muon/_atac/preproc.py:155-236: bounded NMF of the scaled pattern) ---
+ * The reference factorises X [peaks x cells], X[p, c] = s_c where count(c, p) > 0, by coordinate descent.  Every sum
+ * is float64 in a fixed order (per-CTA partials in `workspace`, of mub_scopen_workspace_bytes(rows, k) bytes, summed
+ * in CTA order): every call returns the same bits.  Factors are row-major [rows x k] float64, k <= 64.
+ *   pattern_count : count[i] = entries > 0 of CSR row i (int64 indptr, int32 indices; NaN does not count).
+ *   pattern_fill  : out_indices[out_indptr[i] ..] = the columns of those entries in stored order (out_indptr is the
+ *                   scan of count); with row_scale, out_data[..] = row_scale[i] (fp32, the SVD operand).
+ *   spmm          : C[i, :] = row_scale[i] sum_{j in pattern row i} col_scale[j] B[j, :]; either scale may be NULL
+ *                   (1).  B [cols x k], C [rows x k].
+ *   gram          : G [k x k] = Y^T Y for Y [rows x k].
+ *   cd            : one sweep of sklearn's _update_cdnmf_fast over the rows of W in place, components 0 .. k-1 in
+ *                   order, with HHt = G + l2 I and the update projected onto [0, upper] (upper = +inf: sklearn's);
+ *                   *violation = sum over rows and components of |projected gradient|.
+ *   impute        : out[(p - p0) n + c] = clip(W[p, :] . Ht[c, :], 0, 1) for p0 <= p < p1 (at most 1048560 rows),
+ *                   c < n: a block of rows of clip(W H, 0, 1) [m x n] row-major. */
+#define MUB_SCOPEN_MAX_COMPONENTS 64
+size_t mub_scopen_workspace_bytes(int64_t rows, int32_t k);
+int mub_scopen_pattern_count_f32(const int64_t* indptr, const float* data, int64_t rows, int64_t* count,
+                                 mub_stream_t stream);
+int mub_scopen_pattern_count_f64(const int64_t* indptr, const double* data, int64_t rows, int64_t* count,
+                                 mub_stream_t stream);
+int mub_scopen_pattern_fill_f32(const int64_t* indptr, const int32_t* indices, const float* data, int64_t rows,
+                                const int64_t* out_indptr, const float* row_scale, int32_t* out_indices,
+                                float* out_data, mub_stream_t stream);
+int mub_scopen_pattern_fill_f64(const int64_t* indptr, const int32_t* indices, const double* data, int64_t rows,
+                                const int64_t* out_indptr, const float* row_scale, int32_t* out_indices,
+                                float* out_data, mub_stream_t stream);
+int mub_scopen_spmm_f64(const int64_t* indptr, const int32_t* indices, int64_t rows, const double* row_scale,
+                        const double* col_scale, const double* B, int32_t k, double* C, mub_stream_t stream);
+int mub_scopen_gram_f64(const double* Y, int64_t rows, int32_t k, void* workspace, double* G, mub_stream_t stream);
+int mub_scopen_cd_f64(double* W, int64_t rows, int32_t k, const double* G, double l2, const double* XHt, double upper,
+                      void* workspace, double* violation, mub_stream_t stream);
+int mub_scopen_impute_f64(const double* W, int64_t p0, int64_t p1, const double* Ht, int64_t n, int32_t k,
+                          double* out, mub_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,6 +2,7 @@
 
     import muon_b200 as mu
     mu.atac.pp.tfidf(adata)      # muon/_atac/preproc.py:16
+    mu.atac.pp.scopen(mdata)     # muon/_atac/preproc.py:155  (scOpen; bounded NMF of the peak pattern on the GPU)
     mu.atac.tl.lsi(adata)        # muon/_atac/tools.py:29
     mu.tl.mofa(mdata)            # muon/_core/tools.py:290
     mu.pp.neighbors(mdata)       # muon/_core/preproc.py:264  (WNN; first version, exact search)

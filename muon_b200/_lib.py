@@ -115,6 +115,14 @@ SIGNATURES = {
     "mub_ica_step_f64": [vp, i64, i32, vp, i32, i32, f64, vp, vp, vp],
     "mub_ica_sources_f32": [vp, i64, i32, vp, vp, vp, vp, vp, vp, vp],
     "mub_ica_sources_f64": [vp, i64, i32, vp, vp, vp, vp, vp, vp, vp],
+    "mub_scopen_pattern_count_f32": [vp, vp, i64, vp, vp],
+    "mub_scopen_pattern_count_f64": [vp, vp, i64, vp, vp],
+    "mub_scopen_pattern_fill_f32": [vp, vp, vp, i64, vp, vp, vp, vp, vp],
+    "mub_scopen_pattern_fill_f64": [vp, vp, vp, i64, vp, vp, vp, vp, vp],
+    "mub_scopen_spmm_f64": [vp, vp, i64, vp, vp, vp, i32, vp, vp],
+    "mub_scopen_gram_f64": [vp, i64, i32, vp, vp, vp],
+    "mub_scopen_cd_f64": [vp, i64, i32, vp, f64, vp, f64, vp, vp, vp],
+    "mub_scopen_impute_f64": [vp, i64, i64, vp, i64, i32, vp, vp],
 }
 SPECIAL_RESTYPE = {
     "mub_last_error": ([], C.c_char_p),
@@ -127,6 +135,7 @@ SPECIAL_RESTYPE = {
     "mub_rank_workspace_slice_bytes": ([i32, i32], i64),
     "mub_frag_tile_bytes": ([], i64),
     "mub_ica_workspace_bytes": ([i64, i32, i32], C.c_size_t),
+    "mub_scopen_workspace_bytes": ([i64, i32], C.c_size_t),
 }
 
 TFIDF_LOG_TF, TFIDF_LOG_IDF, TFIDF_LOG_TFIDF, TFIDF_NO_SCALE, TFIDF_BINARIZE = 1, 2, 4, 8, 16
@@ -143,6 +152,7 @@ SNF_DIFFUSE_TRANSPOSED, SNF_DIFFUSE_SYMMETRIC = 0, 1
 MOTIF_MAX_LEN, MOTIF_TILE, MOTIF_CODES, MOTIF_GROUP_COLS = 64, 512, 5, 512
 ICA_MAX_DIM = 128
 ICA_LOGCOSH, ICA_EXP, ICA_CUBE = 0, 1, 2
+SCOPEN_MAX_COMPONENTS = 64
 
 
 class MuonB200Error(RuntimeError):
@@ -181,7 +191,8 @@ KERNELS_PER_CALL = {"mub_csr_transpose_fill_tiled": 2, "mub_csr_transpose_fill":
                     "mub_dsb_moments_f32": 4, "mub_dsb_moments_f64": 4, "mub_dsb_cross_f32": 2, "mub_dsb_cross_f64": 2,
                     "mub_leiden_max_shared_degree": 0,
                     "mub_snf_affinity_f64": 2, "mub_snf_dominate_f64": 2,
-                    "mub_ica_moments_f32": 4, "mub_ica_moments_f64": 4, "mub_ica_step_f64": 2}
+                    "mub_ica_moments_f32": 4, "mub_ica_moments_f64": 4, "mub_ica_step_f64": 2,
+                    "mub_scopen_gram_f64": 2, "mub_scopen_cd_f64": 2}
 LAUNCHES = 0          # running count of kernels launched through this binding
 PROFILE = None        # None, or dict name -> list[(start_event, end_event)] filled by call()
 

@@ -1,4 +1,4 @@
-"""``mu.atac.pp`` -- ATAC preprocessing.  Only ``tfidf`` is on the hot path (SURVEY section 8)."""
+"""``mu.atac.pp`` -- ATAC preprocessing: ``tfidf``, ``binarize`` and ``scopen``."""
 from __future__ import annotations
 
 from typing import Optional, Union
@@ -139,3 +139,16 @@ def binarize(data):
         X.data[X.data != 0] = 1
     else:
         X[X != 0] = 1
+
+
+def scopen(data, n_components: int = 30, max_iter: int = 500, min_rho: float = 0.0, max_rho: float = 0.5,
+           alpha: int = 1, verbose: bool = False):
+    """Impute peak accessibility with scOpen (Li et al., 2019) -- drop-in for ``muon.atac.pp.scopen`` (reference
+    muon/_atac/preproc.py:155-236; same arguments, prints and slots).
+
+    Fills ``obsm["X_scopen"]`` (cells x n_components), ``varm["scopen"]`` (peaks x n_components) and replaces ``X``
+    by the imputed accessibility, a dense float64 cells x peaks matrix in [0, 1].  The bounded NMF runs on the GPU
+    on the sparse pattern of ``X`` (see ``muon_b200._scopen``); at most 64 components are supported."""
+    from .._scopen import scopen as _scopen
+    return _scopen(data, n_components=n_components, max_iter=max_iter, min_rho=min_rho, max_rho=max_rho,
+                   alpha=alpha, verbose=verbose)

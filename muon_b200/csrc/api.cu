@@ -34,7 +34,7 @@ int sm_count() {
 
 extern "C" {
 
-int mub_version(void) { return 108; /* 0.1.8: independent component analysis (ica) */ }
+int mub_version(void) { return 109; /* 0.1.9: scOpen imputation (scopen) */ }
 
 const char* mub_last_error(void) { return mub::g_err; }
 
